@@ -169,10 +169,14 @@ mp_idx_t *mp_idx_restore(const char *fn);                               /* minip
 void mp_idx_print_stat(const mp_idx_t *mi, int32_t max_occ);            /* miniprot.h:285 (index.c:138)   */
 mp_tbuf_t *mp_tbuf_init(void);                                          /* miniprot.h:275 (map.c:16)      */
 void mp_tbuf_destroy(mp_tbuf_t *b);                                     /* miniprot.h:282 (map.c:25)      */
-/* Map one protein: a GPU batch of one.  Return value and r->p / r->feat are malloc'ed (caller frees). */
+/* Map one protein: a GPU batch of one.  Return value and r->p / r->feat are malloc'ed (caller frees).  Safe to call from several
+ * threads at once, as the reference's worker threads do: without MPB_DEVICES the calls take turns on the default context; with
+ * MPB_DEVICES each call takes an idle context of that pool (and waits while all are busy).  ns_global_gs16b does the same. */
 mp_reg1_t *mp_map(const mp_idx_t *mi, int qlen, const char *seq, int *n_reg, mp_tbuf_t *b,
                   const mp_mapopt_t *opt, const char *qname);           /* miniprot.h:268 (map.c:143)     */
-/* Read FASTA proteins from fn, map them in mini-batches on the GPU, write PAF/GFF to stdout in input order. */
+/* Read FASTA proteins from fn, map them in mini-batches on the GPU, write PAF/GFF to stdout in input order.  n_threads is not
+ * used.  MPB_DEVICES=<device>[,<device>...] (read once; repeats allowed, "0,0" = two contexts on device 0) maps the file over one
+ * context per entry (mpb_map_file_multi); the output is the same byte for byte. */
 int32_t mp_map_file(const mp_idx_t *idx, const char *fn, const mp_mapopt_t *opt, int n_threads); /* miniprot.h:286 (map.c:330) */
 double mp_realtime(void);                                               /* mppriv.h:47 (sys.c:93)  */
 double mp_cputime(void);                                                /* mppriv.h:48 (sys.c:107) */
@@ -185,12 +189,15 @@ void mp_set_spsc(const char *fn, mp_idx_t *mi, mp_mapopt_t *mo, int32_t keep_io)
 
 /* ------------------------------------------- (2) GPU batch interface -------------------- */
 
-typedef struct mpb_ctx_s mpb_ctx_t; /* one per process and GPU: stream, device arenas, resident index */
+typedef struct mpb_ctx_s mpb_ctx_t; /* stream, device arenas, resident index; several may share one GPU */
 
-/* Create the context on CUDA device `device`. NULL (with a message on stderr) if there is no device. */
+/* Create the context on CUDA device `device` and keep the calling thread on the device's NUMA node (MPB_AFFINITY=0: leave it).
+ * NULL (with a message on stderr) if there is no device.  Every mpb_* call that uses a context holds the context's mutex, so
+ * calls on one context from several threads take turns; calls on different contexts run concurrently. */
 mpb_ctx_t *mpb_ctx_create(int device);
 void mpb_ctx_destroy(mpb_ctx_t *ctx);
-/* Process-wide default context used by mp_map()/mp_map_file()/ns_global_gs16b(); created on first use. */
+/* Process-wide default context used by mp_map()/mp_map_file()/ns_global_gs16b(); created on first use, on device LOCAL_RANK (or 0),
+ * or on the first device of MPB_DEVICES when that is set (context 0 of the pool). */
 mpb_ctx_t *mpb_ctx_default(void);
 
 /* Make the read-only index resident in HBM (ki, kb, bo, 4-bit genome, contig table). */
@@ -207,6 +214,12 @@ int mpb_idx_device_ptrs(mpb_ctx_t *ctx, void **d_ki, void **d_kb, void **d_seq);
  * uploading from the host (sizes: ki 8*n_bucket, kb 4*n_kb, seq (l_seq+1)/2 bytes). The host-side
  * mp_idx_t must still carry nt->ctg[], bo[], n_kb and opt (small metadata). */
 int mpb_idx_attach_device(mpb_ctx_t *ctx, const mp_idx_t *mi_meta, void *d_ki, void *d_kb, void *d_seq);
+/* Make the index resident in `src` resident in `dst` too; 0, or -1 when src holds none.  On one device dst adopts src's k-mer
+ * tables and genome (nothing is copied); on another device they are copied device to device.  An index loaded with
+ * mpb_idx_load_device reaches other contexts this way (the mapping calls do it themselves when another context holds the index).
+ * A context that adopted must not be in use while the owner of the buffers is destroyed or replaces its index; when that
+ * happens the adopter forgets the index (and shares or uploads it again on its next call). */
+int mpb_idx_share(mpb_ctx_t *dst, mpb_ctx_t *src);
 
 /* Replacement for the reference's kt_for(worker_for) step (map.c:291): map n_seq proteins.
  * reg_out[i] / n_reg_out[i] receive what mp_map() would have returned for protein i.
@@ -221,6 +234,12 @@ int mpb_map_batch(mpb_ctx_t *ctx, const mp_idx_t *mi, const mp_mapopt_t *opt, in
 
 /* mp_map_file() with an explicit output stream and context (tests, benchmarks). */
 int32_t mpb_map_file(mpb_ctx_t *ctx, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, FILE *out);
+/* mpb_map_file() over n_ctx distinct contexts (on one or several GPUs) at once: the input is cut into units of at most
+ * mini_batch_size / n_ctx residues, each context maps the next unit on a thread of its own, and the output is written in input
+ * order -- byte for byte what mpb_map_file() writes.  The index is made resident in every context first (shared from one that holds
+ * it, else uploaded).  Returns what mpb_map_file() returns; -1 also for a repeated or null context.  n_ctx == 1 is mpb_map_file(). */
+int32_t mpb_map_file_multi(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, FILE *out);
+int32_t mpb_map_file_multi_path(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, const char *out_path);
 /* Format one hit exactly like the reference's PAF writer (format.c:333); appends to a malloc'ed buffer. */
 int64_t mpb_format_paf(const mp_idx_t *mi, const mp_mapopt_t *opt, const char *qname, int32_t qlen,
                        const char *qseq, const mp_reg1_t *r, char **buf, int64_t *len, int64_t *cap);

@@ -213,6 +213,12 @@ def lib() -> C.CDLL:
         L.mpb_idx_attach_device.argtypes = [C.c_void_p, C.POINTER(Idx), C.c_void_p, C.c_void_p, C.c_void_p]
         L.mpb_map_file_path.restype = C.c_int32
         L.mpb_map_file_path.argtypes = [C.c_void_p, C.POINTER(Idx), C.c_char_p, C.POINTER(MapOpt), C.c_char_p]
+        L.mpb_map_file_multi_path.restype = C.c_int32
+        L.mpb_map_file_multi_path.argtypes = [C.POINTER(C.c_void_p), C.c_int32, C.POINTER(Idx), C.c_char_p, C.POINTER(MapOpt), C.c_char_p]
+        L.mpb_idx_share.argtypes = [C.c_void_p, C.c_void_p]
+        L.mpb_event_begin.argtypes = [C.c_void_p]
+        L.mpb_event_end_ms.restype = C.c_double
+        L.mpb_event_end_ms.argtypes = [C.c_void_p]
         L.mpb_nasw_batch.argtypes = [C.c_void_p, C.POINTER(NsOpt), C.c_int32, C.POINTER(DpProblem), C.POINTER(DpResult)]
         L.mpb_chain_batch.argtypes = [C.c_void_p, C.POINTER(ChainPar), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.POINTER(C.c_void_p), C.c_void_p, C.POINTER(C.c_void_p)]
@@ -291,6 +297,22 @@ def map_file(ctx: Context, mi, prot_path: str, out_path: str, mo: MapOpt | None 
     rc = lib().mpb_map_file_path(ctx.h, mi, prot_path.encode(), C.byref(mo), out_path.encode())
     if rc != 0:
         raise RuntimeError(f"mpb_map_file failed ({rc})")
+
+
+def idx_share(dst: Context, src: Context) -> None:
+    """mpb_idx_share: make the index resident in `src` resident in `dst` too (adopted on one device, copied device to device
+    otherwise)."""
+    if lib().mpb_idx_share(dst.h, src.h) != 0:
+        raise RuntimeError("mpb_idx_share failed: the source context holds no index")
+
+
+def map_file_multi(ctxs, mi, prot_path: str, out_path: str, mo: MapOpt | None = None) -> None:
+    """mpb_map_file_multi: map_file over several distinct contexts at once (one mapper thread each); same output as map_file."""
+    mo = mo or mapopt()
+    arr = (C.c_void_p * len(ctxs))(*[c.h for c in ctxs])
+    rc = lib().mpb_map_file_multi_path(arr, len(ctxs), mi, prot_path.encode(), C.byref(mo), out_path.encode())
+    if rc != 0:
+        raise RuntimeError(f"mpb_map_file_multi failed ({rc})")
 
 
 def nsopt(mat=None, **over) -> NsOpt:

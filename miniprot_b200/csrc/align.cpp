@@ -8,6 +8,7 @@
 //   finish_region() align.c:331-339  CIGAR assembly + mp_extra_* statistics
 #include <assert.h>
 #include <stdio.h>
+#include <atomic>
 #include "internal.hpp"
 #include "align.hpp"
 
@@ -134,8 +135,8 @@ void RegionPlan::after_wave1(const mp_mapopt_t *opt, const DpSet &w1, std::vecto
 {
 	l_nt = w1.nt_len[(size_t)jobL], l_aa = w1.aa_len[(size_t)jobL];
 	if (l_nt < 0 || (has_right && w1.nt_len[(size_t)jobR] < 0)) { // the stage refused the problem
-		static bool warned = false;
-		if (!warned) fprintf(stderr, "[WARNING] an extension over more than 32767 residues is not supported; such hits are dropped\n"), warned = true;
+		static std::atomic<bool> warned{false}; // several contexts plan on different host threads
+		if (!warned.exchange(true)) fprintf(stderr, "[WARNING] an extension over more than 32767 residues is not supported; such hits are dropped\n");
 		failed = true;
 		return;
 	}

@@ -2,6 +2,7 @@
 // This is the ONLY implementation of the stages in the product: there is no CPU fallback.
 #include <algorithm>
 #include <stdio.h>
+#include <condition_variable>
 #include <mutex>
 #include <sched.h>
 #include "ctx.hpp"
@@ -81,6 +82,9 @@ void build_spsc_table(mpb_ctx_s *c, const mp_idx_t *mi)
 	c->d_ss = c->own_ss.as<uint8_t>(), c->ss_src = nt->spsc, c->ss_l_seq = nt->l_seq;
 }
 
+int acquire_index(mpb_ctx_s *c, const mp_idx_t *mi);
+void pin_to_device_node(int device);
+
 struct CudaStages : Stages {
 	mpb_ctx_s *ctx;
 	explicit CudaStages(mpb_ctx_s *c) : ctx(c) {}
@@ -88,8 +92,13 @@ struct CudaStages : Stages {
 	void need_index(const mp_idx_t *mi)
 	{
 		if (ctx->mi != mi || !ctx->d_seq) {
-			if (mpb_idx_upload(ctx, mi) != 0) { fprintf(stderr, "[miniprot_b200] index upload failed\n"); abort(); }
+			if (acquire_index(ctx, mi) != 0) { fprintf(stderr, "[miniprot_b200] index upload failed\n"); abort(); }
 		}
+	}
+	void thread_init() override
+	{
+		MPB_CUDA_OK(cudaSetDevice(ctx->device));
+		pin_to_device_node(ctx->device);
 	}
 	// residues of the whole batch, concatenated, resident for the duration of the call
 	const Batch *cur_batch = 0; // residues of this batch are already resident (between batch_begin and batch_end)
@@ -212,9 +221,15 @@ void pin_to_device_node(int device)
 	if (n_set > 0) sched_setaffinity(0, sizeof(want), &want);
 }
 
+// Locks, always taken in this order: a context's own mutex (mpb_ctx_s::mu, at the ABI boundary), then g_idx_mu (every change of
+// which index a context holds, so that one context can read another's while it shares it), then g_default_mu (the context list).
 std::mutex g_default_mu;
+std::mutex g_idx_mu;
 mpb_ctx_t *g_default_ctx = 0;
 std::vector<mpb_ctx_s*> g_all_ctx;
+
+// (the --spsc table goes with the index: it is keyed by the address of mi->nt->spsc, which the next index may reuse)
+void forget_index(mpb_ctx_s *c) { c->mi = 0, c->d_seq = 0, c->d_ki = 0, c->d_kb = 0, c->idx_owner = 0, c->ss_src = 0, c->d_ss = 0; }
 
 // an index is identified by its address, so a context must forget it when the host object dies (the next
 // mp_idx_t may be allocated at the same address)
@@ -222,14 +237,26 @@ void on_idx_destroy(const mp_idx_t *mi)
 {
 	std::lock_guard<std::mutex> lk(g_default_mu);
 	for (mpb_ctx_s *c : g_all_ctx)
-		if (c->mi == mi) c->mi = 0, c->d_seq = 0, c->d_ki = 0, c->d_kb = 0;
+		if (c->mi == mi) forget_index(c);
 }
+
+// c is about to overwrite or free its own index buffers: the contexts that adopted them forget the index (they share it again, or
+// upload it, when they next need it).  Under g_idx_mu.
+void forget_adopters(mpb_ctx_s *c)
+{
+	std::lock_guard<std::mutex> lk(g_default_mu);
+	for (mpb_ctx_s *o : g_all_ctx)
+		if (o != c && o->idx_owner == c) forget_index(o);
+}
+
+// Create a context; pin = keep the calling thread on the device's NUMA node (what mpb_ctx_create does for a process per GPU).
+mpb_ctx_s *ctx_new(int device, bool pin);
 
 } // namespace
 
-extern "C" {
+namespace {
 
-mpb_ctx_t *mpb_ctx_create(int device)
+mpb_ctx_s *ctx_new(int device, bool pin)
 {
 	int n_dev = 0;
 	if (cudaGetDeviceCount(&n_dev) != cudaSuccess || n_dev == 0) {
@@ -238,12 +265,14 @@ mpb_ctx_t *mpb_ctx_create(int device)
 	}
 	if (device < 0 || device >= n_dev) { fprintf(stderr, "[miniprot_b200] bad device %d (have %d)\n", device, n_dev); return 0; }
 	MPB_CUDA_OK(cudaSetDevice(device));
-	pin_to_device_node(device);
+	if (pin) pin_to_device_node(device);
 	mpb_ctx_s *c = new mpb_ctx_s();
 	c->device = device;
 	MPB_CUDA_OK(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
 	MPB_CUDA_OK(cudaEventCreate(&c->ev0));
 	MPB_CUDA_OK(cudaEventCreate(&c->ev1));
+	MPB_CUDA_OK(cudaEventCreate(&c->ev_bench[0]));
+	MPB_CUDA_OK(cudaEventCreate(&c->ev_bench[1]));
 	MPB_CUDA_OK(cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming));
 	MPB_CUDA_OK(cudaEventCreateWithFlags(&c->ev_fork2, cudaEventDisableTiming));
 	int prio_lo = 0, prio_hi = 0;
@@ -271,10 +300,171 @@ mpb_ctx_t *mpb_ctx_create(int device)
 	return c;
 }
 
+void upload_meta(mpb_ctx_s *c, const mp_idx_t *mi)
+{
+	const int32_t n_ctg = mi->nt->n_ctg;
+	c->own_bo.reserve(sizeof(uint32_t) * (size_t)(2 * n_ctg + 1));
+	MPB_CUDA_OK(cudaMemcpy(c->own_bo.p, mi->bo, sizeof(uint32_t) * (size_t)(2 * n_ctg + 1), cudaMemcpyHostToDevice));
+	std::vector<int64_t> ctg((size_t)n_ctg * 2);
+	for (int32_t i = 0; i < n_ctg; ++i) ctg[(size_t)i * 2] = mi->nt->ctg[i].off, ctg[(size_t)i * 2 + 1] = mi->nt->ctg[i].len;
+	c->own_ctg.reserve(sizeof(int64_t) * ctg.size() + 16);
+	MPB_CUDA_OK(cudaMemcpy(c->own_ctg.p, ctg.data(), sizeof(int64_t) * ctg.size(), cudaMemcpyHostToDevice));
+	c->d_bo = c->own_bo.as<uint32_t>(), c->d_ctg = c->own_ctg.as<int64_t>();
+}
+
+// mpb_idx_upload without the locks (the caller holds c->mu and g_idx_mu)
+int idx_upload_unlocked(mpb_ctx_s *c, const mp_idx_t *mi)
+{
+	if (!mi->ki || !mi->kb) return c->mi == mi && c->d_ki ? 0 : -1; // loaded straight into HBM: no host tables to upload from (see mpb_idx_share)
+	MPB_CUDA_OK(cudaSetDevice(c->device));
+	forget_adopters(c);
+	const size_t nb = idx_n_bucket(&mi->opt), seq_bytes = (size_t)((mi->nt->l_seq + 1) >> 1);
+	c->own_ki.reserve(sizeof(int64_t) * (nb + 1));
+	c->own_kb.reserve(sizeof(uint32_t) * (size_t)(mi->n_kb + 1));
+	c->own_seq.reserve(seq_bytes + 16);
+	MPB_CUDA_OK(cudaMemcpy(c->own_ki.p, mi->ki, sizeof(int64_t) * nb, cudaMemcpyHostToDevice));
+	MPB_CUDA_OK(cudaMemcpy(c->own_ki.as<int64_t>() + nb, &mi->n_kb, sizeof(int64_t), cudaMemcpyHostToDevice)); // sentinel: end of the last bucket
+	MPB_CUDA_OK(cudaMemcpy(c->own_kb.p, mi->kb, sizeof(uint32_t) * (size_t)mi->n_kb, cudaMemcpyHostToDevice));
+	MPB_CUDA_OK(cudaMemcpy(c->own_seq.p, mi->nt->seq, seq_bytes, cudaMemcpyHostToDevice));
+	c->d_ki = c->own_ki.as<int64_t>(), c->d_kb = c->own_kb.as<uint32_t>(), c->d_seq = c->own_seq.as<uint8_t>();
+	upload_meta(c, mi);
+	c->mi = mi, c->own_index = true, c->idx_owner = 0;
+	c->stats.h2d_bytes += (int64_t)(sizeof(int64_t) * nb + sizeof(uint32_t) * (size_t)mi->n_kb + seq_bytes);
+	return 0;
+}
+
+// mpb_idx_share without the locks (the caller holds dst->mu and g_idx_mu; src's index cannot change meanwhile)
+int idx_share_unlocked(mpb_ctx_s *dst, mpb_ctx_s *src)
+{
+	const mp_idx_t *mi = src->mi;
+	if (!mi || !src->d_ki || !src->d_kb || !src->d_seq) return -1;
+	if (dst == src) return 0;
+	MPB_CUDA_OK(cudaSetDevice(dst->device));
+	if (dst->device == src->device) { // adopt: nothing is copied
+		dst->d_ki = src->d_ki, dst->d_kb = src->d_kb, dst->d_seq = src->d_seq;
+		upload_meta(dst, mi);
+		dst->mi = mi, dst->own_index = false;
+		dst->idx_owner = src->own_index ? src : src->idx_owner; // null: the buffers came from outside (mpb_idx_attach_device)
+		return 0;
+	}
+	// another device: a copy of the three arrays in dst's own buffers, straight from src's (works with or without peer access)
+	forget_adopters(dst);
+	const size_t nb = idx_n_bucket(&mi->opt), seq_bytes = (size_t)((mi->nt->l_seq + 1) >> 1);
+	dst->own_ki.reserve(sizeof(int64_t) * (nb + 1));
+	dst->own_kb.reserve(sizeof(uint32_t) * (size_t)(mi->n_kb + 1));
+	dst->own_seq.reserve(seq_bytes + 16);
+	MPB_CUDA_OK(cudaMemcpyPeerAsync(dst->own_ki.p, dst->device, src->d_ki, src->device, sizeof(int64_t) * (nb + 1), dst->stream)); // with the sentinel
+	if (mi->n_kb) MPB_CUDA_OK(cudaMemcpyPeerAsync(dst->own_kb.p, dst->device, src->d_kb, src->device, sizeof(uint32_t) * (size_t)mi->n_kb, dst->stream));
+	MPB_CUDA_OK(cudaMemcpyPeerAsync(dst->own_seq.p, dst->device, src->d_seq, src->device, seq_bytes, dst->stream));
+	MPB_CUDA_OK(cudaStreamSynchronize(dst->stream));
+	dst->d_ki = dst->own_ki.as<int64_t>(), dst->d_kb = dst->own_kb.as<uint32_t>(), dst->d_seq = dst->own_seq.as<uint8_t>();
+	upload_meta(dst, mi);
+	dst->mi = mi, dst->own_index = true, dst->idx_owner = 0;
+	return 0;
+}
+
+// CudaStages::need_index: the index from another context that holds it (one on the same device first: nothing is copied), else
+// from the host tables.  An index loaded with mpb_idx_load_device has no host tables, so it can only be shared.
+int acquire_index(mpb_ctx_s *c, const mp_idx_t *mi)
+{
+	std::lock_guard<std::mutex> il(g_idx_mu);
+	if (c->mi == mi && c->d_seq) return 0;
+	mpb_ctx_s *src = 0;
+	{
+		std::lock_guard<std::mutex> lk(g_default_mu);
+		for (mpb_ctx_s *o : g_all_ctx)
+			if (o != c && o->mi == mi && o->d_ki && o->d_kb && o->d_seq && (!src || (o->device == c->device && src->device != c->device))) src = o;
+	}
+	return src ? idx_share_unlocked(c, src) : idx_upload_unlocked(c, mi);
+}
+
+// MPB_DEVICES=<device>[,<device>...] (repeats allowed: "0,0" = two contexts on device 0), read once; empty when unset
+const std::vector<int> &pool_devices()
+{
+	static const std::vector<int> dev = [] {
+		std::vector<int> d;
+		const char *e = getenv("MPB_DEVICES");
+		if (!e || !*e) return d;
+		for (const char *q = e; *q;) {
+			char *end;
+			const long v = strtol(q, &end, 10);
+			if (end == q || v < 0 || (*end && *end != ',')) {
+				fprintf(stderr, "[miniprot_b200] MPB_DEVICES=%s: expected a comma-separated list of device numbers\n", e);
+				abort();
+			}
+			d.push_back((int)v);
+			q = *end == ',' ? end + 1 : end;
+		}
+		return d;
+	}();
+	return dev;
+}
+
+// The contexts of MPB_DEVICES: mp_map_file maps over all of them, mp_map and ns_global_gs16b take an idle one.  Context 0 is the
+// default context.  Lives as long as the process.
+class CtxPool {
+public:
+	static CtxPool *get() // null when MPB_DEVICES is unset
+	{
+		static CtxPool *p = pool_devices().empty() ? 0 : new CtxPool();
+		return p;
+	}
+	std::vector<mpb_ctx_s*> ctx;
+	mpb_ctx_s *acquire()
+	{
+		std::unique_lock<std::mutex> lk(mu_);
+		cv_.wait(lk, [&] { return std::find(busy_.begin(), busy_.end(), (char)0) != busy_.end(); });
+		const size_t k = (size_t)(std::find(busy_.begin(), busy_.end(), (char)0) - busy_.begin());
+		busy_[k] = 1;
+		return ctx[k];
+	}
+	void release(mpb_ctx_s *c)
+	{
+		std::lock_guard<std::mutex> lk(mu_);
+		for (size_t k = 0; k < ctx.size(); ++k) if (ctx[k] == c) busy_[k] = 0;
+		cv_.notify_one();
+	}
+
+private:
+	CtxPool()
+	{
+		const std::vector<int> &dev = pool_devices();
+		ctx.push_back(mpb_ctx_default());
+		for (size_t k = 1; k < dev.size(); ++k) {
+			mpb_ctx_s *c = ctx_new(dev[k], false); // the mapper threads keep to the node of their device themselves
+			if (!c) { fprintf(stderr, "[miniprot_b200] MPB_DEVICES: cannot create a context on device %d\n", dev[k]); abort(); }
+			ctx.push_back(c);
+		}
+		busy_.assign(ctx.size(), 0);
+	}
+	std::mutex mu_;
+	std::condition_variable cv_;
+	std::vector<char> busy_;
+};
+
+// one protein on a pool context when MPB_DEVICES is set, else on the default context (whose mutex makes concurrent callers take turns)
+struct AnyCtx {
+	CtxPool *pool = CtxPool::get();
+	mpb_ctx_s *c = pool ? pool->acquire() : mpb_ctx_default();
+	~AnyCtx() { if (pool) pool->release(c); }
+};
+
+} // namespace
+
+extern "C" {
+
+mpb_ctx_t *mpb_ctx_create(int device) { return ctx_new(device, true); }
+
+// A context that adopted another's index buffers (mpb_idx_share on one device) must not be in use while their owner is destroyed
+// or replaces its index.  When that happens the adopter forgets the index, so it never reads freed memory: its next mapping call
+// shares the index again from a context that holds it, or uploads it from the host tables.
 void mpb_ctx_destroy(mpb_ctx_t *c)
 {
 	if (!c) return;
+	std::unique_lock<std::mutex> cl(c->mu);
 	{
+		std::lock_guard<std::mutex> il(g_idx_mu);
+		forget_adopters(c);
 		std::lock_guard<std::mutex> lk(g_default_mu);
 		for (size_t i = 0; i < g_all_ctx.size(); ++i) if (g_all_ctx[i] == c) { g_all_ctx.erase(g_all_ctx.begin() + (ptrdiff_t)i); break; }
 	}
@@ -287,13 +477,17 @@ void mpb_ctx_destroy(mpb_ctx_t *c)
 	c->h_out.release(), c->h_cigar.release();
 	for (PinBuf &b : c->h_c) b.release();
 	cudaEventDestroy(c->ev0), cudaEventDestroy(c->ev1), cudaEventDestroy(c->ev_fork), cudaEventDestroy(c->ev_fork2);
+	cudaEventDestroy(c->ev_bench[0]), cudaEventDestroy(c->ev_bench[1]);
 	for (int i = 0; i < mpb_ctx_s::N_SIDE; ++i) cudaStreamDestroy(c->side[i]), cudaEventDestroy(c->ev_join[i]), cudaEventDestroy(c->ev_k0[i]), cudaEventDestroy(c->ev_k1[i]), cudaEventDestroy(c->ev_km[i]);
 	cudaEventDestroy(c->ev_w0), cudaEventDestroy(c->ev_w1), cudaEventDestroy(c->ev_p0);
 	cudaStreamDestroy(c->stream);
 	delete c->stages;
+	cl.unlock();
 	delete c;
 }
 
+// LOCAL_RANK or device 0; with MPB_DEVICES set, the first device of that list (the default context is context 0 of the pool, and the
+// calling thread is left where it is: the mapper threads keep to their devices' nodes themselves)
 mpb_ctx_t *mpb_ctx_default(void)
 {
 	static std::mutex once_mu; // not g_default_mu: mpb_ctx_create takes that one itself
@@ -301,42 +495,27 @@ mpb_ctx_t *mpb_ctx_default(void)
 	if (!g_default_ctx) {
 		int dev = 0;
 		if (const char *e = getenv("LOCAL_RANK")) dev = atoi(e);
-		g_default_ctx = mpb_ctx_create(dev);
+		const std::vector<int> &pool = pool_devices();
+		g_default_ctx = pool.empty() ? mpb_ctx_create(dev) : ctx_new(pool[0], false);
 		if (!g_default_ctx) { fprintf(stderr, "[miniprot_b200] cannot run without a GPU\n"); abort(); }
 	}
 	return g_default_ctx;
 }
 
-static void upload_meta(mpb_ctx_s *c, const mp_idx_t *mi)
-{
-	const int32_t n_ctg = mi->nt->n_ctg;
-	c->own_bo.reserve(sizeof(uint32_t) * (size_t)(2 * n_ctg + 1));
-	MPB_CUDA_OK(cudaMemcpy(c->own_bo.p, mi->bo, sizeof(uint32_t) * (size_t)(2 * n_ctg + 1), cudaMemcpyHostToDevice));
-	std::vector<int64_t> ctg((size_t)n_ctg * 2);
-	for (int32_t i = 0; i < n_ctg; ++i) ctg[(size_t)i * 2] = mi->nt->ctg[i].off, ctg[(size_t)i * 2 + 1] = mi->nt->ctg[i].len;
-	c->own_ctg.reserve(sizeof(int64_t) * ctg.size() + 16);
-	MPB_CUDA_OK(cudaMemcpy(c->own_ctg.p, ctg.data(), sizeof(int64_t) * ctg.size(), cudaMemcpyHostToDevice));
-	c->d_bo = c->own_bo.as<uint32_t>(), c->d_ctg = c->own_ctg.as<int64_t>();
-}
-
 int mpb_idx_upload(mpb_ctx_t *c, const mp_idx_t *mi)
 {
 	if (!c || !mi) return -1;
-	if (!mi->ki || !mi->kb) return c->mi == mi && c->d_ki ? 0 : -1; // loaded straight into HBM: already resident in its own context, not uploadable elsewhere
-	MPB_CUDA_OK(cudaSetDevice(c->device));
-	const size_t nb = idx_n_bucket(&mi->opt), seq_bytes = (size_t)((mi->nt->l_seq + 1) >> 1);
-	c->own_ki.reserve(sizeof(int64_t) * (nb + 1));
-	c->own_kb.reserve(sizeof(uint32_t) * (size_t)(mi->n_kb + 1));
-	c->own_seq.reserve(seq_bytes + 16);
-	MPB_CUDA_OK(cudaMemcpy(c->own_ki.p, mi->ki, sizeof(int64_t) * nb, cudaMemcpyHostToDevice));
-	MPB_CUDA_OK(cudaMemcpy(c->own_ki.as<int64_t>() + nb, &mi->n_kb, sizeof(int64_t), cudaMemcpyHostToDevice)); // sentinel: end of the last bucket
-	MPB_CUDA_OK(cudaMemcpy(c->own_kb.p, mi->kb, sizeof(uint32_t) * (size_t)mi->n_kb, cudaMemcpyHostToDevice));
-	MPB_CUDA_OK(cudaMemcpy(c->own_seq.p, mi->nt->seq, seq_bytes, cudaMemcpyHostToDevice));
-	c->d_ki = c->own_ki.as<int64_t>(), c->d_kb = c->own_kb.as<uint32_t>(), c->d_seq = c->own_seq.as<uint8_t>();
-	upload_meta(c, mi);
-	c->mi = mi, c->own_index = true;
-	c->stats.h2d_bytes += (int64_t)(sizeof(int64_t) * nb + sizeof(uint32_t) * (size_t)mi->n_kb + seq_bytes);
-	return 0;
+	std::lock_guard<std::mutex> cl(c->mu);
+	std::lock_guard<std::mutex> il(g_idx_mu);
+	return idx_upload_unlocked(c, mi);
+}
+
+int mpb_idx_share(mpb_ctx_t *dst, mpb_ctx_t *src)
+{
+	if (!dst || !src) return -1;
+	std::lock_guard<std::mutex> cl(dst->mu);
+	std::lock_guard<std::mutex> il(g_idx_mu);
+	return idx_share_unlocked(dst, src);
 }
 
 // FASTA -> index with the k-mer tables built on the device (idx_build.cu); called by mp_idx_load through g_idx_build_hook once the
@@ -348,11 +527,16 @@ static int build_index_on_device(mp_idx_t *mi)
 	int n_dev = 0;
 	if (cudaGetDeviceCount(&n_dev) != cudaSuccess || n_dev <= 0) { cudaGetLastError(); return -1; }
 	mpb_ctx_t *c = mpb_ctx_default();
+	std::lock_guard<std::mutex> cl(c->mu);
+	std::lock_guard<std::mutex> il(g_idx_mu);
+	MPB_CUDA_OK(cudaSetDevice(c->device));
 	const double t0 = mp_realtime();
+	forget_adopters(c);
+	if (c->own_index) forget_index(c); // the build reuses the context's own buffers
 	if (idx_build_device(c, mi) != 0) return -1;
 	c->d_ki = c->own_ki.as<int64_t>(), c->d_kb = c->own_kb.as<uint32_t>(), c->d_seq = c->own_seq.as<uint8_t>();
 	upload_meta(c, mi);
-	c->mi = mi, c->own_index = true;
+	c->mi = mi, c->own_index = true, c->idx_owner = 0;
 	if (mp_verbose >= 3) fprintf(stderr, "[M::%s@%.3f] built the k-mer tables on the device in %.3f s: %ld kmer-block pairs\n", __func__, mp_realtime(), mp_realtime() - t0, (long)mi->n_kb);
 	return 0;
 }
@@ -365,11 +549,15 @@ namespace { struct IdxBuildHook { IdxBuildHook() { mpb::g_idx_build_hook = build
 mp_idx_t *mpb_idx_load_device(mpb_ctx_t *c, const char *fn)
 {
 	if (!c || !fn) return 0;
+	std::lock_guard<std::mutex> cl(c->mu);
+	std::lock_guard<std::mutex> il(g_idx_mu);
 	MPB_CUDA_OK(cudaSetDevice(c->device));
 	FILE *fp = fopen(fn, "rb");
 	if (!fp) return 0;
 	mp_idx_t *mi = idx_restore_head(fp);
 	if (!mi) { fclose(fp); return 0; }
+	forget_adopters(c);
+	if (c->own_index) forget_index(c); // its buffers are refilled below
 	const size_t nb = idx_n_bucket(&mi->opt), seq_bytes = (size_t)((mi->nt->l_seq + 1) >> 1);
 	c->own_ki.reserve(sizeof(int64_t) * (nb + 1));
 	c->own_kb.reserve(sizeof(uint32_t) * (size_t)(mi->n_kb + 1));
@@ -402,7 +590,7 @@ mp_idx_t *mpb_idx_load_device(mpb_ctx_t *c, const char *fn)
 	if (!ok) { mp_idx_destroy(mi); return 0; }
 	c->d_ki = c->own_ki.as<int64_t>(), c->d_kb = c->own_kb.as<uint32_t>(), c->d_seq = c->own_seq.as<uint8_t>();
 	upload_meta(c, mi);
-	c->mi = mi, c->own_index = true;
+	c->mi = mi, c->own_index = true, c->idx_owner = 0;
 	c->stats.h2d_bytes += (int64_t)(sizeof(int64_t) * nb + sizeof(uint32_t) * (size_t)mi->n_kb + seq_bytes);
 	if (mp_verbose >= 3) fprintf(stderr, "[M::%s@%.3f] loaded the index into device memory\n", __func__, mp_realtime());
 	return mi;
@@ -422,7 +610,9 @@ mp_idx_t *mpb_idx_load_meta(const char *fn)
 // device addresses of the resident index of a context (the source buffers of the broadcast on the rank that loaded the file)
 int mpb_idx_device_ptrs(mpb_ctx_t *c, void **d_ki, void **d_kb, void **d_seq)
 {
-	if (!c || !c->d_ki) return -1;
+	if (!c) return -1;
+	std::lock_guard<std::mutex> cl(c->mu);
+	if (!c->d_ki) return -1;
 	*d_ki = c->d_ki, *d_kb = c->d_kb, *d_seq = c->d_seq;
 	return 0;
 }
@@ -430,10 +620,12 @@ int mpb_idx_device_ptrs(mpb_ctx_t *c, void **d_ki, void **d_kb, void **d_seq)
 int mpb_idx_attach_device(mpb_ctx_t *c, const mp_idx_t *mi, void *d_ki, void *d_kb, void *d_seq)
 {
 	if (!c || !mi || !d_ki || !d_kb || !d_seq) return -1;
+	std::lock_guard<std::mutex> cl(c->mu);
+	std::lock_guard<std::mutex> il(g_idx_mu);
 	MPB_CUDA_OK(cudaSetDevice(c->device));
 	c->d_ki = (int64_t*)d_ki, c->d_kb = (uint32_t*)d_kb, c->d_seq = (uint8_t*)d_seq;
 	upload_meta(c, mi);
-	c->mi = mi, c->own_index = false;
+	c->mi = mi, c->own_index = false, c->idx_owner = 0;
 	return 0;
 }
 
@@ -442,6 +634,7 @@ int mpb_map_batch(mpb_ctx_t *c, const mp_idx_t *mi, const mp_mapopt_t *opt, int3
 {
 	if (!c) return -1;
 	if (bad_scoring(opt->go, opt->ie_coef) || bad_index(mi)) return -3;
+	std::lock_guard<std::mutex> cl(c->mu);
 	MPB_CUDA_OK(cudaSetDevice(c->device));
 	Batch b;
 	b.n = n_seq, b.seq = seqs, b.len = lens, b.name = names;
@@ -453,6 +646,7 @@ int32_t mpb_map_file(mpb_ctx_t *c, const mp_idx_t *mi, const char *fn, const mp_
 {
 	if (!c) return -1;
 	if (bad_scoring(opt->go, opt->ie_coef) || bad_index(mi)) return -3;
+	std::lock_guard<std::mutex> cl(c->mu);
 	MPB_CUDA_OK(cudaSetDevice(c->device));
 	return map_file(c->stages, mi, fn, opt, out);
 }
@@ -466,17 +660,49 @@ int32_t mpb_map_file_path(mpb_ctx_t *c, const mp_idx_t *mi, const char *fn, cons
 	return rc;
 }
 
+int32_t mpb_map_file_multi(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, FILE *out)
+{
+	if (!ctx || n_ctx < 1) return -1;
+	std::vector<mpb_ctx_s*> by_addr(ctx, ctx + n_ctx);
+	std::sort(by_addr.begin(), by_addr.end());
+	if (by_addr[0] == 0 || std::adjacent_find(by_addr.begin(), by_addr.end()) != by_addr.end()) return -1; // a context maps one unit at a time
+	if (n_ctx == 1) return mpb_map_file(ctx[0], mi, fn, opt, out);
+	if (bad_scoring(opt->go, opt->ie_coef) || bad_index(mi)) return -3;
+	std::vector<std::unique_lock<std::mutex>> held;
+	for (mpb_ctx_s *c : by_addr) held.emplace_back(c->mu); // in address order: two such calls never wait for each other in a cycle
+	// the index is resident in every context before the mappers start: in the first one that holds it or can upload it, shared
+	// from there to the others (on the same device nothing is copied)
+	for (int32_t k = 0; k < n_ctx; ++k) {
+		if (ctx[k]->mi == mi && ctx[k]->d_seq) continue;
+		if (acquire_index(ctx[k], mi) != 0) { fprintf(stderr, "[miniprot_b200] the index is neither resident in a context nor on the host\n"); return -1; }
+	}
+	std::vector<Stages*> st((size_t)n_ctx);
+	for (int32_t k = 0; k < n_ctx; ++k) st[(size_t)k] = ctx[k]->stages;
+	return map_file_multi(st.data(), n_ctx, mi, fn, opt, out);
+}
+
+int32_t mpb_map_file_multi_path(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, const char *out_path)
+{
+	FILE *fp = fopen(out_path, "wb");
+	if (!fp) return -2;
+	int32_t rc = mpb_map_file_multi(ctx, n_ctx, mi, fn, opt, fp);
+	fclose(fp);
+	return rc;
+}
+
 mp_reg1_t *mp_map(const mp_idx_t *mi, int qlen, const char *seq, int *n_reg, mp_tbuf_t *, const mp_mapopt_t *opt, const char *qname)
 {
 	mp_reg1_t *reg = 0;
 	int32_t len = qlen, nr = 0;
-	mpb_map_batch(mpb_ctx_default(), mi, opt, 1, &seq, &len, &qname, &nr, &reg);
+	AnyCtx a;
+	mpb_map_batch(a.c, mi, opt, 1, &seq, &len, &qname, &nr, &reg);
 	*n_reg = nr;
 	return reg;
 }
 
 int32_t mp_map_file(const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, int)
 {
+	if (CtxPool *p = CtxPool::get()) return mpb_map_file_multi(p->ctx.data(), (int32_t)p->ctx.size(), mi, fn, opt, stdout);
 	return mpb_map_file(mpb_ctx_default(), mi, fn, opt, stdout);
 }
 
@@ -494,6 +720,7 @@ int mpb_nasw_batch(mpb_ctx_t *c, const ns_opt_t *opt, int32_t n, const mpb_dp_pr
 {
 	if (!c) return -1;
 	if (bad_scoring(opt->go, opt->ie_coef)) return -3;
+	std::lock_guard<std::mutex> cl(c->mu);
 	MPB_CUDA_OK(cudaSetDevice(c->device));
 	// pack the host sequences the way the genome is stored, so that the same kernels serve both paths
 	int64_t nt_tot = 0, aa_tot = 0;
@@ -549,6 +776,7 @@ int mpb_chain_batch(mpb_ctx_t *c, const mpb_chain_par_t *par, int32_t n, const i
                     uint64_t **b)
 {
 	if (!c) return -1;
+	std::lock_guard<std::mutex> cl(c->mu);
 	MPB_CUDA_OK(cudaSetDevice(c->device));
 	chn::Par p;
 	p.max_dist_x = par->max_dist_x, p.max_dist_y = par->max_dist_y, p.bw = par->bw, p.max_skip = par->max_skip, p.max_iter = par->max_iter;
@@ -567,6 +795,7 @@ int mpb_chain_batch(mpb_ctx_t *c, const mpb_chain_par_t *par, int32_t n, const i
 int mpb_seed_batch(mpb_ctx_t *c, const mp_idx_t *mi, int32_t max_occ, int32_t n_seq, const char *const *seqs, const int32_t *lens, int64_t *a_off, uint64_t **a)
 {
 	if (c == 0 || mi == 0 || n_seq < 0) return -1;
+	std::lock_guard<std::mutex> cl(c->mu);
 	MPB_CUDA_OK(cudaSetDevice(c->device));
 	Batch b;
 	b.n = n_seq, b.seq = seqs, b.len = lens, b.name = 0;
@@ -587,6 +816,7 @@ int mpb_refine_batch(mpb_ctx_t *c, const mp_idx_t *mi, const mp_mapopt_t *opt, i
                      const mpb_window_t *win, int64_t *a_off, uint64_t **a, int32_t *sc)
 {
 	if (c == 0 || mi == 0 || opt == 0 || n_seq < 0 || n_win < 0) return -1;
+	std::lock_guard<std::mutex> cl(c->mu);
 	MPB_CUDA_OK(cudaSetDevice(c->device));
 	Batch b;
 	b.n = n_seq, b.seq = seqs, b.len = lens, b.name = 0;
@@ -608,6 +838,7 @@ int mpb_refine_batch(mpb_ctx_t *c, const mp_idx_t *mi, const mp_mapopt_t *opt, i
 int mpb_sort_segments(mpb_ctx_t *c, int32_t n_seg, const int64_t *off, uint64_t *keys)
 {
 	if (!c || n_seg < 0) return -1;
+	std::lock_guard<std::mutex> cl(c->mu);
 	MPB_CUDA_OK(cudaSetDevice(c->device));
 	const size_t N = n_seg ? (size_t)off[n_seg] : 0;
 	if (N == 0) return 0;
@@ -630,21 +861,23 @@ void mpb_regs_free(int32_t n, const int32_t *n_reg, mp_reg1_t **reg) // what the
 	}
 }
 
-// CUDA-event bracket on the context's stream (bench.py times its K steps with these)
-static cudaEvent_t g_bench_ev[2];
+// CUDA-event bracket on the context's stream (bench.py times its K steps with these); each context has its own pair of events, on
+// its own device
 void mpb_event_begin(mpb_ctx_t *c)
 {
+	std::lock_guard<std::mutex> cl(c->mu);
 	MPB_CUDA_OK(cudaSetDevice(c->device));
-	if (!g_bench_ev[0]) { MPB_CUDA_OK(cudaEventCreate(&g_bench_ev[0])); MPB_CUDA_OK(cudaEventCreate(&g_bench_ev[1])); }
 	MPB_CUDA_OK(cudaStreamSynchronize(c->stream));
-	MPB_CUDA_OK(cudaEventRecord(g_bench_ev[0], c->stream));
+	MPB_CUDA_OK(cudaEventRecord(c->ev_bench[0], c->stream));
 }
 double mpb_event_end_ms(mpb_ctx_t *c)
 {
+	std::lock_guard<std::mutex> cl(c->mu);
 	float ms = 0;
-	MPB_CUDA_OK(cudaEventRecord(g_bench_ev[1], c->stream));
-	MPB_CUDA_OK(cudaEventSynchronize(g_bench_ev[1]));
-	MPB_CUDA_OK(cudaEventElapsedTime(&ms, g_bench_ev[0], g_bench_ev[1]));
+	MPB_CUDA_OK(cudaSetDevice(c->device));
+	MPB_CUDA_OK(cudaEventRecord(c->ev_bench[1], c->stream));
+	MPB_CUDA_OK(cudaEventSynchronize(c->ev_bench[1]));
+	MPB_CUDA_OK(cudaEventElapsedTime(&ms, c->ev_bench[0], c->ev_bench[1]));
 	return ms;
 }
 
@@ -653,7 +886,8 @@ void ns_global_gs16b(void *, const char *ns, int32_t nl, const char *as, int32_t
 	mpb_dp_problem_t p;
 	mpb_dp_result_t o;
 	p.nt = (const uint8_t*)ns, p.aa = as, p.ss = ss, p.nl = nl, p.al = al, p.flag = opt->flag, p.io = opt->io;
-	if (mpb_nasw_batch(mpb_ctx_default(), opt, 1, &p, &o) != 0) abort();
+	AnyCtx a;
+	if (mpb_nasw_batch(a.c, opt, 1, &p, &o) != 0) abort();
 	r->score = o.score, r->nt_len = o.nt_len, r->aa_len = o.aa_len;
 	r->n_cigar = r->m_cigar = o.n_cigar, r->cigar = o.cigar;
 	if (!(opt->flag & (NS_F_EXT_LEFT | NS_F_EXT_RIGHT))) r->nt_len = nl, r->aa_len = al;
@@ -664,7 +898,15 @@ void ns_global_gs16(void *km, const char *ns, int32_t nl, const char *as, int32_
 	ns_global_gs16b(km, ns, nl, as, al, opt, 0, r);
 }
 
-void mpb_get_stats(const mpb_ctx_t *c, mpb_stats_t *st) { *st = c->stats; }
-void mpb_reset_stats(mpb_ctx_t *c) { memset(&c->stats, 0, sizeof(c->stats)); }
+void mpb_get_stats(const mpb_ctx_t *c, mpb_stats_t *st)
+{
+	std::lock_guard<std::mutex> cl(c->mu);
+	*st = c->stats;
+}
+void mpb_reset_stats(mpb_ctx_t *c)
+{
+	std::lock_guard<std::mutex> cl(c->mu);
+	memset(&c->stats, 0, sizeof(c->stats));
+}
 
 } // extern "C"

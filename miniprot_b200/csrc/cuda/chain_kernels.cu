@@ -11,6 +11,7 @@
 #include <cuda_runtime.h>
 #include "chain_core.cuh"
 #include "chain_dev.hpp"
+#include "smem_attr.hpp"
 
 namespace mpb {
 namespace cuda {
@@ -498,8 +499,8 @@ void chain_launch_smem(cudaStream_t st, const int32_t *list, int n_list, int cap
 {
 	if (n_list <= 0) return;
 	const int smem = cap * 16 + 16;
-	static int attr_max = 0;
-	if (smem > attr_max) { cudaFuncSetAttribute(chain_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); attr_max = smem; }
+	static SmemLimit lim; // raised on demand, per device
+	lim.raise(chain_smem_kernel, smem);
 	chain_smem_kernel<<<n_list, 32, smem, st>>>(list, n_list, cap, a_off, cnt, a, par, v, (FlagRange<uint64_t>*)stack, u, b, n_u, n_b, resort);
 }
 
@@ -508,8 +509,8 @@ void chain_launch_bt_smem(cudaStream_t st, const int32_t *list, int n_list, int 
 {
 	if (n_list <= 0) return;
 	const int smem = cap * 13 + 16;
-	static int attr_max = 0;
-	if (smem > attr_max) { cudaFuncSetAttribute(chain_bt_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); attr_max = smem; }
+	static SmemLimit lim; // raised on demand, per device
+	lim.raise(chain_bt_smem_kernel, smem);
 	chain_bt_smem_kernel<<<n_list, 32, smem, st>>>(list, n_list, cap, a_off, cnt, a, par, f, p, v, (FlagRange<uint64_t>*)stack, u, b, n_u, n_b, resort);
 }
 

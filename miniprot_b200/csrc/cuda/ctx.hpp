@@ -1,5 +1,6 @@
 // ctx.hpp -- the per-process, per-GPU context behind mpb_ctx_t (host side of the CUDA backend).
 #pragma once
+#include <mutex>
 #include <vector>
 #include "../internal.hpp"
 #include "devbuf.hpp"
@@ -7,8 +8,12 @@
 
 struct mpb_ctx_s {
 	int device = 0;
+	// taken by every mpb_* entry point that uses the context: concurrent calls on one context take turns (the stream, the arenas
+	// and the resident index are the context's alone).  Internal paths below an entry point never take it again.
+	mutable std::mutex mu;
 	cudaStream_t stream = 0;
 	cudaEvent_t ev0 = 0, ev1 = 0;
+	cudaEvent_t ev_bench[2] = {0, 0}; // mpb_event_begin / mpb_event_end_ms
 	// side streams: size classes of one DP wave (and independent stage pieces) run concurrently; each class is bounded
 	// by its longest problem, so serialising them on one stream would add the critical paths up
 	static const int N_SIDE = 32; // 0..8 are high-priority streams (extension classes of a DP wave: their long problems must be dispatched first; 3, the widest class, highest), 9..17 normal
@@ -16,8 +21,9 @@ struct mpb_ctx_s {
 	cudaEvent_t ev_fork = 0, ev_fork2 = 0, ev_join[N_SIDE] = {0}, ev_k0[N_SIDE] = {0}, ev_k1[N_SIDE] = {0}, ev_km[N_SIDE] = {0};
 	cudaEvent_t ev_w0 = 0, ev_w1 = 0, ev_p0 = 0; // timing of a DP wave on the main stream: before the prep kernel, at the fork, after the last join
 
-	// resident read-only index (uploaded once, or adopted from an NCCL broadcast)
+	// resident read-only index (uploaded once, adopted from an NCCL broadcast, or shared by another context: mpb_idx_share)
 	const mp_idx_t *mi = 0;
+	mpb_ctx_s *idx_owner = 0; // the context whose ki / kb / seq buffers this one adopted (same device), else null
 	uint8_t *d_seq = 0;       // 4-bit genome, (l_seq+1)/2 bytes
 	int64_t *d_ki = 0;        // n_bucket + 1 entries (a sentinel n_kb is appended on upload)
 	uint32_t *d_kb = 0;

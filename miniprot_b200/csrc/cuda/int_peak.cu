@@ -70,6 +70,7 @@ extern "C" int mpb_int_peak(mpb_ctx_t *c, int variant, double *thread_instr_per_
 {
 	using namespace mpb::cuda;
 	if (!c || variant < 0 || variant > 4) return -1;
+	std::lock_guard<std::mutex> lk(c->mu);
 	MPB_CUDA_OK(cudaSetDevice(c->device));
 	cudaDeviceProp pr;
 	MPB_CUDA_OK(cudaGetDeviceProperties(&pr, c->device));

@@ -33,11 +33,27 @@ static inline int pick_C(int al)
 // family for everything (A/B measurements and tests only).
 // Per nucleotide row the block-wide kernel is the faster one, and a mini-batch is latency bound -- its waves last as long as
 // their longest problem (100 k-row extensions).
-static int g_forced_family = 0; // MPB_NASW_KERNEL=cols|v3 (A/B switch for tests and measurements), read once per nasw_run
-static inline bool use_v3(int al, int nl)
+// The A/B switches of the dispatcher are read from the environment at every nasw_run into a value of its own (tests switch the
+// family between calls), never into a global: DP waves of several contexts run concurrently on different host threads.
+struct Switches {
+	int forced_family = 0; // MPB_NASW_KERNEL=cols|v3|pair (A/B switch for tests and measurements): 1, 2, 3
+	int pass_warps = 8;
+	int wide_warps = 4;    // passes of a problem wider than 256 columns: 128 columns each (MPB_NASW_WIDE_WARPS=8: 256)
+	bool split_long = false; // MPB_NASW_SPLIT=1: long extensions of 129..256 columns as two 4-warp column passes (measured slower, see below)
+	static Switches from_env()
+	{
+		Switches s;
+		const char *e = getenv("MPB_NASW_KERNEL"), *pw = getenv("MPB_NASW_PASS_WARPS"), *ww = getenv("MPB_NASW_WIDE_WARPS"), *sp = getenv("MPB_NASW_SPLIT");
+		s.pass_warps = pw && atoi(pw) == 2 ? 2 : 8;
+		s.wide_warps = ww && atoi(ww) == 8 ? 8 : 4;
+		s.split_long = sp && atoi(sp) != 0;
+		s.forced_family = !e ? 0 : strcmp(e, "cols") == 0 ? 1 : strcmp(e, "v3") == 0 ? 2 : strcmp(e, "pair") == 0 ? 3 : 0;
+		return s;
+	}
+};
+static inline bool use_v3(const Switches &sw)
 {
-	(void)al, (void)nl;
-	return g_forced_family != 1; // default: latency first (a wave is bounded by its longest problems); wide problems run in passes
+	return sw.forced_family != 1; // default: latency first (a wave is bounded by its longest problems); wide problems run in passes
 }
 // Warps per CTA of the block-wide kernels.  A problem wider than one CTA (256 columns) runs as column PASSES, one CTA per pass,
 // all passes of a problem concurrently (pass q a few dozen rows behind pass q - 1, linked by a per-row carry array and a progress
@@ -46,17 +62,14 @@ static inline bool use_v3(int al, int nl)
 // publishing fence, the carry traffic and above all the start-up lag of each further pass (short global alignments!) cost more
 // than that gains over a whole C2 step, so CTAs of up to 8 warps stay the default.
 constexpr int NCLS_ = 13;
-static int g_pass_warps = 8;
-static int g_wide_warps = 4; // passes of a problem wider than 256 columns: 128 columns each (MPB_NASW_WIDE_WARPS=8: 256)
-static bool g_split_long = false; // MPB_NASW_SPLIT=1: long extensions of 129..256 columns as two 4-warp column passes (measured slower, see below)
-static inline int v3_warps(int al)
+static inline int v3_warps(const Switches &sw, int al)
 {
 	const int nw = ((al + 7) / 8 * 8 + 31) / 32;
 	const int r = nw <= 1 ? 1 : nw <= 2 ? 2 : nw <= 4 ? 4 : 8;
 	// wider than one CTA anyway: passes of 128 columns (four warps meet at the barrier of a macro-step instead of eight, which on
 	// 350 columns x 100 k rows beats two 8-warp passes)
-	if (nw > 8 && g_wide_warps < 8) return g_wide_warps;
-	return r < g_pass_warps ? r : g_pass_warps;
+	if (nw > 8 && sw.wide_warps < 8) return sw.wide_warps;
+	return r < sw.pass_warps ? r : sw.pass_warps;
 }
 
 // Pair-lane kernels (nasw_pair.cuh: two columns per thread as packed int16x2) serve every problem whose scores provably stay
@@ -67,13 +80,13 @@ static nsw::PairLimits pair_limits(const ns_opt_t *o) { return nsw::pair_limits(
 // Score-only extensions stay on the block-wide kernels: there the pair-lane form needs more cycles per row -- its 64 columns per
 // warp do not pay for the 32-bit row-maximum bookkeeping that an extension carries per cell.  MPB_NASW_KERNEL=pair sends every
 // problem of up to 64 columns to them (tests, A/B).
-static inline bool use_pair(const DpDev &j, const ns_opt_t *o, const nsw::PairLimits &l)
+static inline bool use_pair(const Switches &sw, const DpDev &j, const ns_opt_t *o, const nsw::PairLimits &l)
 {
-	if (g_forced_family == 1 || g_forced_family == 2) return false;
+	if (sw.forced_family == 1 || sw.forced_family == 2) return false;
 	const int W8 = (j.al + 7) / 8 * 8;
 	if (W8 > nsw::PAIR_MAX_W8 || j.nl < 3) return false;
 	if (j.ss_off >= 0) return false; // --spsc makes donor / acceptor entries negative: outside the value-domain argument of the pair-lane kernels
-	if (g_forced_family != 3) {
+	if (sw.forced_family != 3) {
 		const bool is_tb = !(j.flag & (NS_F_EXT_LEFT | NS_F_EXT_RIGHT));
 		if (!is_tb) return false;
 	}
@@ -103,7 +116,8 @@ int nasw_check_ie_coef(float ie_coef)
 }
 
 // run jobs[lo, hi) as one sub-wave
-static void run_subwave(mpb_ctx_s *ctx, const uint8_t *packed, const uint8_t *d_ss, const char *d_aa, const NaswConst &cst, const ns_opt_t *nso, std::vector<DpDev> &jobs, size_t lo, size_t hi, DpSet &out)
+static void run_subwave(mpb_ctx_s *ctx, const Switches &sw, const uint8_t *packed, const uint8_t *d_ss, const char *d_aa, const NaswConst &cst, const ns_opt_t *nso,
+                        std::vector<DpDev> &jobs, size_t lo, size_t hi, DpSet &out)
 {
 	const int n = (int)(hi - lo);
 	if (n == 0) return;
@@ -125,7 +139,7 @@ static void run_subwave(mpb_ctx_s *ctx, const uint8_t *packed, const uint8_t *d_
 			j.C = 0, j.pad_ = 32, j.rw_off = 0, j.tb_off = j.cig_off = 0, j.cig_cap = 0, j.carry_off = 0;
 			continue;
 		}
-		if (use_pair(j, nso, plim)) { // pair-lane kernels: pair records (96 B per triple of rows), wavefront-major traceback of 64 columns per warp
+		if (use_pair(sw, j, nso, plim)) { // pair-lane kernels: pair records (96 B per triple of rows), wavefront-major traceback of 64 columns per warp
 			const int W8 = (j.al + 7) / 8 * 8, K = nsw::pair_rec_slots(j.nl), n_macro = nsw::pair_n_macro(j.nl, W8);
 			j.C = 0, j.pad_ = 64;
 			j.rw_off = rw_tot, rw_tot += (int64_t)192 * nsw::pair_rec_blocks(j.nl); // two parities x blocks x 192 sixteen-byte fields, in units of 32 bytes
@@ -142,12 +156,12 @@ static void run_subwave(mpb_ctx_s *ctx, const uint8_t *packed, const uint8_t *d_
 			(is_tb ? ctx->stats.n_dp_tb : ctx->stats.n_dp_ext) += 1;
 			continue;
 		}
-		const bool v3 = use_v3(j.al, j.nl);
-		int nw = v3_warps(j.al);
+		const bool v3 = use_v3(sw);
+		int nw = v3_warps(sw, j.al);
 		// A long extension of 129..256 columns is a pole of its wave on one 8-warp CTA (eight warps at one barrier).  Two concurrent
 		// column passes of four warps (fewer cycles per row each, linked by the carry row; class 10) looked like the way out and are NOT:
 		// on C2 the pass pipeline costs about twice the rows of a lone CTA, as it does for the 350-column problems that need it.  Opt-in only.
-		const bool split = g_split_long && v3 && !is_tb && nw == 8 && j.nl >= 32768 && (j.al + 7) / 8 * 8 <= 256 && (j.al + 7) / 8 * 8 > 128;
+		const bool split = sw.split_long && v3 && !is_tb && nw == 8 && j.nl >= 32768 && (j.al + 7) / 8 * 8 <= 256 && (j.al + 7) / 8 * 8 > 128;
 		if (split) nw = 4;
 		j.C = v3 ? 0 : pick_C(j.al);
 		j.pad_ = v3 ? 32 * nw : 0;
@@ -363,14 +377,7 @@ void nasw_run(mpb_ctx_s *ctx, const uint8_t *packed, const uint8_t *d_ss, const 
 	out.score.assign(n, 0), out.nt_len.assign(n, 0), out.aa_len.assign(n, 0);
 	out.cig.clear(), out.cig_off.assign(n + 1, 0);
 	if (n == 0) return;
-	{
-		const char *e = getenv("MPB_NASW_KERNEL");
-		const char *pw = getenv("MPB_NASW_PASS_WARPS");
-		g_pass_warps = pw && atoi(pw) == 2 ? 2 : 8;
-		{ const char *ww = getenv("MPB_NASW_WIDE_WARPS"); g_wide_warps = ww && atoi(ww) == 8 ? 8 : 4; }
-		if (const char *sp = getenv("MPB_NASW_SPLIT")) g_split_long = atoi(sp) != 0; else g_split_long = false;
-		g_forced_family = !e ? 0 : strcmp(e, "cols") == 0 ? 1 : strcmp(e, "v3") == 0 ? 2 : strcmp(e, "pair") == 0 ? 3 : 0;
-	}
+	const Switches sw = Switches::from_env();
 	NaswConst cst;
 	fill_const(base, cst);
 	size_t lo = 0;
@@ -379,13 +386,13 @@ void nasw_run(mpb_ctx_s *ctx, const uint8_t *packed, const uint8_t *d_ss, const 
 		while (hi < n) {
 			const DpDev &j = jobs[hi];
 			const bool is_tb = !(j.flag & (NS_F_EXT_LEFT | NS_F_EXT_RIGHT));
-			const bool v3 = use_v3(j.al, j.nl);
-			const int C = pick_C(j.al), Wp = v3 ? 32 * v3_warps(j.al) : 32 * C, W8 = (j.al + 7) / 8 * 8, n_pass = (W8 + Wp - 1) / Wp;
+			const bool v3 = use_v3(sw);
+			const int C = pick_C(j.al), Wp = v3 ? 32 * v3_warps(sw, j.al) : 32 * C, W8 = (j.al + 7) / 8 * 8, n_pass = (W8 + Wp - 1) / Wp;
 			const size_t tbb = is_tb ? (size_t)n_pass * (size_t)(j.nl + 3 * Wp + 64) * Wp * 2 : 0, rwb = (size_t)(j.nl + 20) * 32;
 			if (hi > lo && (tb_bytes + tbb > kTbBudget || rw_bytes + rwb > kRwBudget)) break;
 			tb_bytes += tbb, rw_bytes += rwb, ++hi;
 		}
-		run_subwave(ctx, packed, d_ss, d_aa, cst, base, jobs, lo, hi, out);
+		run_subwave(ctx, sw, packed, d_ss, d_aa, cst, base, jobs, lo, hi, out);
 		lo = hi;
 	}
 }

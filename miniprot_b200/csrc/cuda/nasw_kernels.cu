@@ -22,6 +22,7 @@
 #include "nasw_core.cuh"
 #include "nasw_dev.hpp"
 #include "nasw_warp.cuh"
+#include "smem_attr.hpp"
 
 namespace mpb {
 namespace cuda {
@@ -546,8 +547,8 @@ template <int C, bool MULTI>
 static void launch_ext(cudaStream_t st, const DpDev *jobs, const int *order, int n, const int4 *rec, const char *aa, const NaswConst &cst, int4 *out, int *carry)
 {
 	const int smem = NASW_WARPS * 22 * 32 * C * (int)sizeof(int);
-	static bool attr_set = false;
-	if (!attr_set) { cudaFuncSetAttribute(nasw_ext_kernel<C, MULTI>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); attr_set = true; }
+	static SmemLimit lim;
+	lim.raise(nasw_ext_kernel<C, MULTI>, smem);
 	nasw_ext_kernel<C, MULTI><<<(n + NASW_WARPS - 1) / NASW_WARPS, NASW_WARPS * 32, smem, st>>>(jobs, order, n, rec, aa, cst, out, carry);
 }
 
@@ -556,8 +557,8 @@ static void launch_tb(cudaStream_t st, const DpDev *jobs, const int *order, int 
                       uint16_t *tb)
 {
 	const int smem = NASW_WARPS * 22 * 32 * C * (int)sizeof(int);
-	static bool attr_set = false;
-	if (!attr_set) { cudaFuncSetAttribute(nasw_tb_kernel<C, MULTI>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); attr_set = true; }
+	static SmemLimit lim;
+	lim.raise(nasw_tb_kernel<C, MULTI>, smem);
 	nasw_tb_kernel<C, MULTI><<<(n + NASW_WARPS - 1) / NASW_WARPS, NASW_WARPS * 32, smem, st>>>(jobs, order, n, rec, aa, cst, out, carry, tb);
 }
 
@@ -603,13 +604,13 @@ static void launch_v3(cudaStream_t st, const DpDev *jobs, const int *order, int 
 {
 	int smem = 22 * 32 * NW * (int)sizeof(int);
 	if (warps_per_sm > 0) {
-		static int stat = -1;
-		if (stat < 0) {
+		static const int stat = [] { // static shared memory of the kernel: the same on every device of the one architecture built for
 			cudaFuncAttributes fa;
 			cudaFuncGetAttributes(&fa, nasw_v3_kernel<NW, TB, MP>);
-			stat = ((int)fa.sharedSizeBytes + 15) & ~15;
-			cudaFuncSetAttribute(nasw_v3_kernel<NW, TB, MP>, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448 - stat);
-		}
+			return ((int)fa.sharedSizeBytes + 15) & ~15;
+		}();
+		static SmemLimit lim;
+		lim.raise(nasw_v3_kernel<NW, TB, MP>, 232448 - stat);
 		const int share = (int)((int64_t)233472 * NW / warps_per_sm) - 1024 - stat;
 		smem = std::max(smem, std::min(share, 232448 - stat)) & ~15;
 	}

@@ -17,6 +17,7 @@
 #include <vector>
 #include "ctx.hpp"
 #include "seed_dev.hpp"
+#include "smem_attr.hpp"
 
 namespace mpb {
 namespace cuda {
@@ -132,11 +133,8 @@ void seg_sort_u64(mpb_ctx_s *ctx, cudaStream_t st, uint64_t *keys, uint64_t *tmp
 	MPB_CUDA_OK(cudaMemcpyAsync(ctx->b_c[3].p, all.data(), sizeof(SegDesc) * all.size(), cudaMemcpyHostToDevice, st));
 	// (a copy from pageable memory has left the host buffer when the call returns)
 	const SegDesc *d_small = ctx->b_c[3].as<SegDesc>(), *d_single = d_small + small.size(), *d_mtile = d_single + single.size(), *d_mchunk = d_mtile + mtile.size();
-	static bool attr_set = false;
-	if (!attr_set) {
-		cudaFuncSetAttribute(seg_tile_sort_kernel<SORT_TILE, 1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, SORT_TILE * 8);
-		attr_set = true;
-	}
+	static SmemLimit lim;
+	lim.raise(seg_tile_sort_kernel<SORT_TILE, 1024>, SORT_TILE * 8);
 	if (u_small) seg_tile_sort_kernel<SORT_SMALL, 256><<<u_small, 256, SORT_SMALL * 8, st>>>(d_small, (int)small.size(), keys, keys), ctx->stats.kernel_launches += 1;
 	if (u_single) seg_tile_sort_kernel<SORT_TILE, 1024><<<u_single, 1024, SORT_TILE * 8, st>>>(d_single, (int)single.size(), keys, keys), ctx->stats.kernel_launches += 1;
 	if (u_mtile) {

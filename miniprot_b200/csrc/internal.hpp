@@ -104,11 +104,16 @@ struct Stages {
 	virtual void batch_end() {}
 	// wall-clock accounting of the dispatcher's phases (0 S1, 1 H1, 2 S2, 3 H2, 4 S3 waves, 5 H3); optional
 	virtual void note_wall(int /*phase*/, double /*ms*/) {}
+	// called on a host thread before it first calls the stages (the mapper threads of map_file_multi): a device backend makes its
+	// device current there and keeps the thread on the device's NUMA node; optional
+	virtual void thread_init() {}
 };
 
 // ---------------------------------------------------------------- host pipeline (pipeline.cpp, hits.cpp, align.cpp)
 void map_batch(Stages *st, const mp_idx_t *mi, const mp_mapopt_t *opt, const Batch &b, int32_t *n_reg_out, mp_reg1_t **reg_out);
 int32_t map_file(Stages *st, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, FILE *out);
+// map_file over n backends at once (one mapper thread each); n == 1 is map_file.  The stages must be distinct.
+int32_t map_file_multi(Stages *const *st, int n, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, FILE *out);
 
 struct Str {                      // growable output buffer
 	char *s = 0; int64_t l = 0, m = 0;

@@ -16,6 +16,8 @@
 #include <algorithm>
 #include <chrono>
 #include <condition_variable>
+#include <deque>
+#include <map>
 #include <memory>
 #include <mutex>
 #include <thread>
@@ -370,6 +372,93 @@ int32_t map_file(Stages *st, const mp_idx_t *mi, const char *fn, const mp_mapopt
 	}
 	to_write.close();
 	reader.join();
+	writer.join();
+	return 0;
+}
+
+// map_file over n backends (contexts, possibly on several devices): one reader thread cuts the input into work units of at most
+// mini_batch_size / n residues (at least one protein; results do not depend on batch boundaries), n mapper threads -- one per
+// backend -- take the next unit each, and one writer thread emits the units strictly in input order and owns the hit counter, as
+// in map_file.  At most 2n units are between the reader and the writer, so memory stays bounded whatever the input.
+// The host phases of the mappers share one worker pool and take turns on it (parfor.hpp), the device stages overlap.
+int32_t map_file_multi(Stages *const *st, int n, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, FILE *out)
+{
+	if (n < 1) return -1;
+	if (n == 1) return map_file(st[0], mi, fn, opt, out);
+	FastxReader rd(fn);
+	if (!rd.fp) return -1;
+	if (opt->flag & MP_F_GFF) fputs("##gff-version 3\n", out); // map.c:338
+	const int64_t unit_size = std::max<int64_t>(1, opt->mini_batch_size / n);
+	const int64_t max_in_flight = 2 * (int64_t)n;
+	static const bool trace = getenv("MPB_TRACE") != 0;
+
+	std::mutex mu;
+	std::condition_variable cv;
+	std::deque<std::pair<int64_t, std::unique_ptr<FileBatch>>> todo; // read, not yet taken by a mapper
+	std::map<int64_t, std::unique_ptr<FileBatch>> mapped;              // mapped, not yet written
+	int64_t n_read = 0, n_written = 0;                                   // units
+	bool eof = false;
+
+	std::thread reader([&] {
+		bool more = true;
+		while (more) {
+			{
+				std::unique_lock<std::mutex> lk(mu);
+				cv.wait(lk, [&] { return n_read - n_written < max_in_flight; });
+			}
+			std::unique_ptr<FileBatch> fb = read_batch(rd, unit_size, more);
+			const bool last = !fb || !more;
+			std::lock_guard<std::mutex> lk(mu);
+			if (fb) todo.emplace_back(n_read++, std::move(fb));
+			if (last) eof = true;
+			cv.notify_all();
+		}
+	});
+	std::vector<std::thread> mappers;
+	for (int k = 0; k < n; ++k)
+		mappers.emplace_back([&, k] {
+			st[k]->thread_init();
+			for (;;) {
+				std::pair<int64_t, std::unique_ptr<FileBatch>> u;
+				{
+					std::unique_lock<std::mutex> lk(mu);
+					cv.wait(lk, [&] { return !todo.empty() || eof; });
+					if (todo.empty()) return;
+					u = std::move(todo.front());
+					todo.pop_front();
+				}
+				FileBatch &fb = *u.second;
+				map_batch(st[k], mi, opt, fb.view(), fb.n_reg.data(), fb.reg.data());
+				if (mp_verbose >= 3)
+					fprintf(stderr, "[M::%s::%.3f*%.2f] mapped %d sequences (context %d)\n", "map_file_multi", mp_realtime(), mp_cputime() / mp_realtime(), (int)fb.seqs.size(), k);
+				std::lock_guard<std::mutex> lk(mu);
+				mapped.emplace(u.first, std::move(u.second));
+				cv.notify_all();
+			}
+		});
+	std::thread writer([&] {
+		int64_t id_counter = 0;
+		for (;;) {
+			std::unique_ptr<FileBatch> fb;
+			{
+				std::unique_lock<std::mutex> lk(mu);
+				cv.wait(lk, [&] { return mapped.count(n_written) || (eof && n_written == n_read); });
+				auto it = mapped.find(n_written);
+				if (it == mapped.end()) return; // everything read has been written
+				fb = std::move(it->second);
+				mapped.erase(it);
+			}
+			const double t0 = mp_realtime();
+			write_batch(out, mi, opt, fb->view(), fb->n_reg.data(), fb->reg.data(), &id_counter);
+			fb->release();
+			if (trace) fprintf(stderr, "[mpb-trace] output: unit %ld, %d proteins formatted + written in %.2f ms\n", (long)n_written, (int)fb->seqs.size(), (mp_realtime() - t0) * 1e3);
+			std::lock_guard<std::mutex> lk(mu);
+			++n_written;
+			cv.notify_all();
+		}
+	});
+	reader.join();
+	for (std::thread &t : mappers) t.join();
 	writer.join();
 	return 0;
 }
