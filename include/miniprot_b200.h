@@ -34,6 +34,14 @@
 #define MP_F_SHOW_TRANS   0x100
 #define MP_F_NO_CS        0x200
 
+/* mp_dbg_flag bits, set by the CLI's debugging switches (reference mppriv.h:9-14, main.c:162-167); read once per mapping call */
+#define MP_DBG_NO_KALLOC   0x1  /* --no-kalloc: allocator choice of the reference; nothing to do here */
+#define MP_DBG_QNAME       0x2  /* --dbg-qname: "QR\tname\tlen\ttid" on stderr before each protein (file and batch calls, not mp_map) */
+#define MP_DBG_NO_REFINE   0x4  /* --dbg-no-refine: no second-round refinement; needs MP_F_NO_ALIGN (-A), refused (-3) without */
+#define MP_DBG_MORE_DP     0x8  /* --dbg-aflt: no seed filter, one global DP over the whole region instead of fills between anchors */
+#define MP_DBG_ANCHOR      0x10 /* --dbg-anchor: "X" lines, every seed anchor of the protein, on stderr */
+#define MP_DBG_CHAIN       0x20 /* --dbg-chain: "Y1" lines, the anchors of every first-round region, on stderr */
+
 #define MP_FEAT_CDS  0
 #define MP_FEAT_STOP 1
 #define MP_IDX_MAGIC "MPI\3"

@@ -234,6 +234,20 @@ def lib() -> C.CDLL:
     return _lib
 
 
+# mp_dbg_flag bits (include/miniprot_b200.h MP_DBG_*; the CLI's --dbg-* switches, reference mppriv.h:9-14)
+DBG_NO_KALLOC, DBG_QNAME, DBG_NO_REFINE, DBG_MORE_DP, DBG_ANCHOR, DBG_CHAIN = 0x1, 0x2, 0x4, 0x8, 0x10, 0x20
+DBG_SWITCHES = {"--no-kalloc": DBG_NO_KALLOC, "--dbg-qname": DBG_QNAME, "--dbg-no-refine": DBG_NO_REFINE, "--dbg-aflt": DBG_MORE_DP,
+                "--dbg-anchor": DBG_ANCHOR, "--dbg-chain": DBG_CHAIN}
+
+
+def set_dbg_flag(bits: int, L: C.CDLL | None = None) -> int:
+    """Set mp_dbg_flag (what main.c's --dbg-* switches set) in the library, or in `L` -- another library built from the same host
+    sources; returns the previous value.  The mapping calls read it once per batch."""
+    v = C.c_int32.in_dll(L or lib(), "mp_dbg_flag")
+    old, v.value = v.value, bits
+    return old
+
+
 def n_bucket(io: IdxOpt) -> int:
     return 1 << (io.kmer * 4 - io.mod_bit)
 

@@ -84,15 +84,17 @@ Fill RegionPlan::make_fill(const mp_idx_t *mi, const mp_mapopt_t *opt, const cha
 }
 
 bool RegionPlan::plan(const mp_idx_t *mi, const mp_mapopt_t *opt, int32_t qid_, int32_t qlen_, const char *aa, mp_reg1_t *r_, int32_t extl0, int32_t extr0,
-                      std::vector<DpJob> &jobs)
+                      bool whole_, std::vector<DpJob> &jobs)
 {
-	r = r_, qid = qid_, qlen = qlen_;
+	r = r_, qid = qid_, qlen = qlen_, whole = whole_;
 	jobL = jobL2 = jobR = jobR2 = -1;
 	fills.clear();
-	mark_tight_anchors(r->cnt, r->a, 6, 3, opt->kmer2, opt->kmer2 + 1);
 	int32_t i0 = 0;
-	while (i0 < r->cnt && !(r->a[i0] >> 31 & 1)) ++i0;
-	if (i0 == r->cnt) { r->cnt = 0; return false; } // align.c:252-255: nothing to pin the alignment
+	if (!whole) { // --dbg-aflt: every anchor counts, the left extension starts from the first one (align.c:248)
+		mark_tight_anchors(r->cnt, r->a, 6, 3, opt->kmer2, opt->kmer2 + 1);
+		while (i0 < r->cnt && !(r->a[i0] >> 31 & 1)) ++i0;
+		if (i0 == r->cnt) { r->cnt = 0; return false; } // align.c:252-255: nothing to pin the alignment
+	}
 	int32_t extl = opt->max_ext, extr = opt->max_ext;
 	if (r->qs >= 10) extl = opt->max_intron / 2;
 	if (qlen - r->qe >= 10) extr = opt->max_intron / 2;
@@ -111,14 +113,17 @@ bool RegionPlan::plan(const mp_idx_t *mi, const mp_mapopt_t *opt, int32_t qid_, 
 		jobL = (int32_t)jobs.size();
 		jobs.push_back(j);
 	}
-	int32_t ne0 = (int32_t)(r->a[i0] >> 32) + 1, ae0 = as1;
-	for (int32_t i = i0 + 1; i < r->cnt; ++i) { // align.c:306-312
-		if (!(r->a[i] >> 31 & 1)) continue;
-		const int32_t ne1 = (int32_t)(r->a[i] >> 32) + 1, ae1 = (int32_t)(r->a[i] & 0x7fffffffU) + 1;
-		fills.push_back(make_fill(mi, opt, aa, ne0, ne1, ae0, ae1, jobs));
-		ne0 = ne1, ae0 = ae1;
+	if (whole) ve_pin = r->ve, qe_pin = r->qe; // align.c:303-304: the region keeps the end its refined chain gave it
+	else {
+		int32_t ne0 = (int32_t)(r->a[i0] >> 32) + 1, ae0 = as1;
+		for (int32_t i = i0 + 1; i < r->cnt; ++i) { // align.c:306-312
+			if (!(r->a[i] >> 31 & 1)) continue;
+			const int32_t ne1 = (int32_t)(r->a[i] >> 32) + 1, ae1 = (int32_t)(r->a[i] & 0x7fffffffU) + 1;
+			fills.push_back(make_fill(mi, opt, aa, ne0, ne1, ae0, ae1, jobs));
+			ne0 = ne1, ae0 = ae1;
+		}
+		ve_pin = ne0 + vs0, qe_pin = ae0;
 	}
-	ve_pin = ne0 + vs0, qe_pin = ae0;
 	// align.c:316.  With fewer than 3 bases left the reference's extension loop never runs and it stops at an assertion
 	// (nasw-sse.c:443); such a hit simply ends at the last pinned anchor here.
 	has_right = qe_pin < qlen && ve_pin < ae && ae - ve_pin >= 3;
@@ -166,8 +171,10 @@ void RegionPlan::after_retry(const mp_idx_t *mi, const mp_mapopt_t *opt, const c
 	if (jobR2 >= 0 && w1r.aa_len[(size_t)jobR2] == qlen - qe_pin) r_nt = w1r.nt_len[(size_t)jobR2], r_aa = w1r.aa_len[(size_t)jobR2];
 	r->vs = vs1 - l_nt;
 	r->qs = as1 - l_aa;
-	// the span found by the left extension, aligned globally to get its CIGAR (first pass of the loop at align.c:306)
-	left_fill = make_fill(mi, opt, aa, (int32_t)(r->vs - vs0), (int32_t)(vs1 - vs0), r->qs, as1, jobs2);
+	// the span found by the left extension, aligned globally to get its CIGAR (first pass of the loop at align.c:306); with
+	// --dbg-aflt the whole region from there to its end (align.c:304)
+	if (whole) left_fill = make_fill(mi, opt, aa, (int32_t)(r->vs - vs0), (int32_t)(ve_pin - vs0), r->qs, qe_pin, jobs2);
+	else left_fill = make_fill(mi, opt, aa, (int32_t)(r->vs - vs0), (int32_t)(vs1 - vs0), r->qs, as1, jobs2);
 	if (has_right) // align.c:331
 		right_fill = make_fill(mi, opt, aa, (int32_t)(ve_pin - vs0), (int32_t)(ve_pin - vs0) + r_nt, qe_pin, qe_pin + r_aa, jobs2);
 }
@@ -277,6 +284,15 @@ static void fill_statistics(const mp_idx_t *mi, mp_reg1_t *r, const mp_mapopt_t 
 void RegionPlan::finish(const mp_idx_t *mi, const mp_mapopt_t *opt, const char *aa, const DpSet &w1, const DpSet &w2)
 {
 	if (failed) { r->p = 0; return; }
+	auto refused = [&](const Fill &f, const DpSet &src) { return !f.ungapped && f.job >= 0 && src.nt_len[(size_t)f.job] < 0; };
+	bool any_refused = refused(left_fill, w2) || (has_right && refused(right_fill, w2));
+	for (size_t i = 0; i < fills.size() && !any_refused; ++i) any_refused = refused(fills[i], w1);
+	if (any_refused) { // the stage could not run a global alignment: its traceback does not fit the free device memory
+		static std::atomic<bool> warned{false};
+		if (!warned.exchange(true)) fprintf(stderr, "[WARNING] a global alignment whose traceback does not fit the free device memory was not run; such hits are dropped\n");
+		r->p = 0;
+		return;
+	}
 	std::vector<uint32_t> cg;
 	int32_t score = 0;
 	auto take = [&](const Fill &f, const DpSet &src) {

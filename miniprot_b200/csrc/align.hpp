@@ -25,7 +25,9 @@ struct RegionPlan {
 	int64_t ve_pin = 0;       // end of the last pinned anchor
 	int32_t qe_pin = 0;
 	bool has_right = false;
-	bool failed = false;      // a DP problem of this region could not be run (extension over more than 32767 residues): the region is dropped
+	bool whole = false;       // --dbg-aflt (align.c:248,303): no seed filter, one global DP from the extended start to the region's end
+	bool failed = false;      // a DP problem of this region could not be run (extension over more than 32767 residues, or a whole-region
+	                          // traceback larger than the free device memory): the region is dropped
 	int32_t jobL = -1, jobL2 = -1, jobR = -1, jobR2 = -1;
 	int32_t l_nt = 0, l_aa = 0, r_nt = 0, r_aa = 0; // accepted extension results
 	Fill left_fill, right_fill; // wave 2
@@ -33,8 +35,8 @@ struct RegionPlan {
 
 	Fill make_fill(const mp_idx_t *mi, const mp_mapopt_t *opt, const char *aa, int32_t ne0, int32_t ne1, int32_t ae0, int32_t ae1,
 	               std::vector<DpJob> &jobs) const;
-	// returns false when the region has no pinned anchor and is dropped
-	bool plan(const mp_idx_t *mi, const mp_mapopt_t *opt, int32_t qid, int32_t qlen, const char *aa, mp_reg1_t *r, int32_t extl0, int32_t extr0,
+	// returns false when the region has no pinned anchor and is dropped; whole = --dbg-aflt (MP_DBG_MORE_DP)
+	bool plan(const mp_idx_t *mi, const mp_mapopt_t *opt, int32_t qid, int32_t qlen, const char *aa, mp_reg1_t *r, int32_t extl0, int32_t extr0, bool whole,
 	          std::vector<DpJob> &jobs);
 	// wave-1 job indices were taken in a list that is appended to the wave's list at position d
 	void rebase_wave1(int32_t d)

@@ -629,23 +629,30 @@ int mpb_idx_attach_device(mpb_ctx_t *c, const mp_idx_t *mi, void *d_ki, void *d_
 	return 0;
 }
 
-int mpb_map_batch(mpb_ctx_t *c, const mp_idx_t *mi, const mp_mapopt_t *opt, int32_t n_seq, const char *const *seqs, const int32_t *lens,
-                  const char *const *names, int32_t *n_reg_out, mp_reg1_t **reg_out)
+// mpb_map_batch; qr_tid < 0: no QR lines of --dbg-qname (mp_map, which the reference calls after printing them in worker_for)
+static int map_batch_on(mpb_ctx_t *c, const mp_idx_t *mi, const mp_mapopt_t *opt, int32_t n_seq, const char *const *seqs, const int32_t *lens,
+                        const char *const *names, int32_t *n_reg_out, mp_reg1_t **reg_out, int32_t qr_tid)
 {
 	if (!c) return -1;
-	if (bad_scoring(opt->go, opt->ie_coef) || bad_index(mi)) return -3;
+	if (bad_scoring(opt->go, opt->ie_coef) || bad_index(mi) || bad_dbg_flags(opt)) return -3;
 	std::lock_guard<std::mutex> cl(c->mu);
 	MPB_CUDA_OK(cudaSetDevice(c->device));
 	Batch b;
 	b.n = n_seq, b.seq = seqs, b.len = lens, b.name = names;
-	map_batch(c->stages, mi, opt, b, n_reg_out, reg_out);
+	map_batch(c->stages, mi, opt, b, n_reg_out, reg_out, qr_tid);
 	return 0;
+}
+
+int mpb_map_batch(mpb_ctx_t *c, const mp_idx_t *mi, const mp_mapopt_t *opt, int32_t n_seq, const char *const *seqs, const int32_t *lens,
+                  const char *const *names, int32_t *n_reg_out, mp_reg1_t **reg_out)
+{
+	return map_batch_on(c, mi, opt, n_seq, seqs, lens, names, n_reg_out, reg_out, 0);
 }
 
 int32_t mpb_map_file(mpb_ctx_t *c, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, FILE *out)
 {
 	if (!c) return -1;
-	if (bad_scoring(opt->go, opt->ie_coef) || bad_index(mi)) return -3;
+	if (bad_scoring(opt->go, opt->ie_coef) || bad_index(mi) || bad_dbg_flags(opt)) return -3;
 	std::lock_guard<std::mutex> cl(c->mu);
 	MPB_CUDA_OK(cudaSetDevice(c->device));
 	return map_file(c->stages, mi, fn, opt, out);
@@ -667,7 +674,7 @@ int32_t mpb_map_file_multi(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_idx_t 
 	std::sort(by_addr.begin(), by_addr.end());
 	if (by_addr[0] == 0 || std::adjacent_find(by_addr.begin(), by_addr.end()) != by_addr.end()) return -1; // a context maps one unit at a time
 	if (n_ctx == 1) return mpb_map_file(ctx[0], mi, fn, opt, out);
-	if (bad_scoring(opt->go, opt->ie_coef) || bad_index(mi)) return -3;
+	if (bad_scoring(opt->go, opt->ie_coef) || bad_index(mi) || bad_dbg_flags(opt)) return -3;
 	std::vector<std::unique_lock<std::mutex>> held;
 	for (mpb_ctx_s *c : by_addr) held.emplace_back(c->mu); // in address order: two such calls never wait for each other in a cycle
 	// the index is resident in every context before the mappers start: in the first one that holds it or can upload it, shared
@@ -695,7 +702,7 @@ mp_reg1_t *mp_map(const mp_idx_t *mi, int qlen, const char *seq, int *n_reg, mp_
 	mp_reg1_t *reg = 0;
 	int32_t len = qlen, nr = 0;
 	AnyCtx a;
-	mpb_map_batch(a.c, mi, opt, 1, &seq, &len, &qname, &nr, &reg);
+	map_batch_on(a.c, mi, opt, 1, &seq, &len, &qname, &nr, &reg, -1);
 	*n_reg = nr;
 	return reg;
 }

@@ -392,7 +392,22 @@ void nasw_run(mpb_ctx_s *ctx, const uint8_t *packed, const uint8_t *d_ss, const 
 			if (hi > lo && (tb_bytes + tbb > kTbBudget || rw_bytes + rwb > kRwBudget)) break;
 			tb_bytes += tbb, rw_bytes += rwb, ++hi;
 		}
+		// A problem over the budget runs in a sub-wave of its own (a whole-region alignment of --dbg-aflt over a long region).  It runs
+		// only when the device has the memory for its arenas (the current ones are freed before they grow; reserve() adds a quarter);
+		// otherwise it reports nt_len = -1 and the caller drops its region with a warning, instead of failing in cudaMalloc.
+		const bool oversize = tb_bytes > kTbBudget || rw_bytes > kRwBudget;
+		if (oversize) {
+			size_t free_b = 0, total_b = 0;
+			MPB_CUDA_OK(cudaMemGetInfo(&free_b, &total_b));
+			const size_t need = (tb_bytes + rw_bytes) / 4 * 5 + ((size_t)1 << 30), have = free_b + ctx->b_tb.cap + ctx->b_rw.cap;
+			if (need > have) {
+				for (size_t k = lo; k < hi; ++k) out.score[k] = INT32_MIN, out.nt_len[k] = -1, out.aa_len[k] = 0, out.cig_off[k + 1] = (int64_t)out.cig.size();
+				lo = hi;
+				continue;
+			}
+		}
 		run_subwave(ctx, sw, packed, d_ss, d_aa, cst, base, jobs, lo, hi, out);
+		if (oversize) ctx->b_tb.release(), ctx->b_rw.release(); // not kept past the budget: other contexts on the device need the memory
 		lo = hi;
 	}
 }

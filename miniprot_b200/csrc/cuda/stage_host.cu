@@ -240,6 +240,13 @@ void seed_chain_run(mpb_ctx_s *ctx, const mp_idx_t *mi, const mp_mapopt_t *opt, 
 	uint64_t *d_a = 0;
 	int64_t *d_a_off = 0;
 	seed_run(ctx, mi, opt->max_occ, b, aa_off, d_aa, a_off, &d_a, &d_a_off);
+	if (out.want_seeds) { // --dbg-anchor: the sorted seeds, before the chaining stages reuse the buffers
+		out.seed_off = a_off;
+		out.seed.resize((size_t)a_off[(size_t)n_q]);
+		if (!out.seed.empty()) MPB_CUDA_OK(cudaMemcpyAsync(out.seed.data(), d_a, sizeof(uint64_t) * out.seed.size(), cudaMemcpyDeviceToHost, ctx->stream));
+		MPB_CUDA_OK(cudaStreamSynchronize(ctx->stream));
+		ctx->stats.d2h_bytes += (int64_t)(sizeof(uint64_t) * out.seed.size());
+	}
 	const int32_t w = 1 << mi->opt.bbit, spl = !(opt->flag & MP_F_NO_SPLICE);
 	const chn::Par pre = chain_par(w, w, w, opt, 2, 0, mi->opt.kmer, mi->opt.bbit);
 	const chn::Par mainp = chain_par(opt->max_intron, opt->max_gap, opt->bw, opt, opt->min_chn_cnt, opt->min_chn_sc, mi->opt.kmer, mi->opt.bbit);

@@ -60,6 +60,11 @@ struct ChainSet {                // result of one chaining stage over many probl
 	std::vector<int64_t> a_off;  // [n+1] into a
 	std::vector<uint64_t> u;     // score<<32 | n_anchors, per chain (chain.c:160 *_u)
 	std::vector<uint64_t> a;     // compacted anchors
+	// --dbg-anchor (map.c:179-184): set by the caller of seed_chain to have the seeds of each query returned as well -- sorted,
+	// max_occ-filtered, before any chaining -- in seed[seed_off[q], seed_off[q+1]).  Left empty otherwise.
+	bool want_seeds = false;
+	std::vector<int64_t> seed_off;
+	std::vector<uint64_t> seed;
 };
 
 struct RefineJob {               // one second-round window (map.c:32-47)
@@ -93,7 +98,7 @@ struct DpSet {
 
 struct Stages {
 	virtual ~Stages() {}
-	// map.c:155-195: sketch, lookup, sort, pre-chain, main chain -- per query
+	// map.c:155-195: sketch, lookup, sort, pre-chain, main chain -- per query; the seeds too when out.want_seeds is set
 	virtual void seed_chain(const mp_idx_t *mi, const mp_mapopt_t *opt, const Batch &b, ChainSet &out) = 0;
 	// map.c:41-97 per window
 	virtual void refine(const mp_idx_t *mi, const mp_mapopt_t *opt, const Batch &b, const std::vector<RefineJob> &jobs, RefineSet &out) = 0;
@@ -110,7 +115,13 @@ struct Stages {
 };
 
 // ---------------------------------------------------------------- host pipeline (pipeline.cpp, hits.cpp, align.cpp)
-void map_batch(Stages *st, const mp_idx_t *mi, const mp_mapopt_t *opt, const Batch &b, int32_t *n_reg_out, mp_reg1_t **reg_out);
+// The --dbg-* switches (mp_dbg_flag, MP_DBG_*) are read once per call.  Their dumps go to stderr, one contiguous block per batch:
+// per protein a QR line (only when qr_tid >= 0; the reference prints it in worker_for, map.c:268, so mp_map prints none), its X
+// lines and its Y1 lines.  qr_tid is the tid field of the QR lines: the index of the context that maps the batch.
+void map_batch(Stages *st, const mp_idx_t *mi, const mp_mapopt_t *opt, const Batch &b, int32_t *n_reg_out, mp_reg1_t **reg_out, int32_t qr_tid = -1);
+// --dbg-no-refine without -A: the reference aligns regions that have no refined anchors and crashes (mp_align, r->a == NULL).
+// True, with a message on stderr, when mp_dbg_flag and opt ask for that: the callers then map nothing and return -3.
+bool bad_dbg_flags(const mp_mapopt_t *opt);
 int32_t map_file(Stages *st, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, FILE *out);
 // map_file over n backends at once (one mapper thread each); n == 1 is map_file.  The stages must be distinct.
 int32_t map_file_multi(Stages *const *st, int n, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, FILE *out);

@@ -14,6 +14,7 @@
 // Results per protein are identical to mp_map() (no state crosses proteins: SURVEY 8b "determinism contract").
 #include <stdio.h>
 #include <algorithm>
+#include <atomic>
 #include <chrono>
 #include <condition_variable>
 #include <deque>
@@ -37,11 +38,60 @@ struct QueryState {
 	std::vector<uint64_t> ext;
 };
 
+template <class... T> void put_fmt(Str &s, const char *fmt, T... v)
+{
+	char line[1024];
+	const int l = snprintf(line, sizeof(line), fmt, v...);
+	if (l < (int)sizeof(line)) s.put(line, l);
+	else {
+		std::vector<char> big((size_t)l + 1);
+		snprintf(big.data(), big.size(), fmt, v...);
+		s.put(big.data(), l);
+	}
+}
+
+// map.c:179-184: the seeds of one protein, with contig, strand and offset of their block
+void dump_seeds(Str &s, const mp_idx_t *mi, int64_t n, const uint64_t *a)
+{
+	for (int64_t k = 0; k < n; ++k) {
+		const uint64_t blk = a[k] >> 32;
+		const int32_t v = idx_block2vid(mi, (uint32_t)blk);
+		put_fmt(s, "X\t%ld\t%s\t%c\t%ld\t%d\n", (long)blk, mi->nt->ctg[v >> 1].name, "+-"[v & 1], (long)((blk - mi->bo[v]) << mi->opt.bbit), (int32_t)(uint32_t)a[k]);
+	}
+}
+
+// map.c:113-124 (mp_dbg_chain, label Y1): every anchor counted by a first-round region, offset from the block of its strand.  A chain
+// cut at a contig boundary still counts the anchors of the side it lost, and they print with the kept strand's first block: the
+// difference may be negative, and is computed as the reference's 64-bit wrap-around.
+void dump_chains(Str &s, const mp_idx_t *mi, int32_t n_reg, const mp_reg1_t *reg, const uint64_t *a)
+{
+	for (int32_t i = 0; i < n_reg; ++i) {
+		const mp_reg1_t *r = &reg[i];
+		for (int32_t k = 0; k < r->cnt; ++k) {
+			const uint64_t ak = a[r->off + k];
+			const int64_t off = (int64_t)(((ak >> 32) - (uint64_t)mi->bo[r->vid]) << mi->opt.bbit);
+			put_fmt(s, "Y1\t%d\t%ld\t%s\t%c\t%ld\t%d\n", i, (long)(ak >> 32), mi->nt->ctg[r->vid >> 1].name, "+-"[r->vid & 1], (long)off, (int32_t)(uint32_t)ak);
+		}
+	}
+}
+
 } // namespace
 
-void map_batch(Stages *st, const mp_idx_t *mi, const mp_mapopt_t *opt, const Batch &b, int32_t *n_reg_out, mp_reg1_t **reg_out)
+bool bad_dbg_flags(const mp_mapopt_t *opt)
+{
+	if (!(mp_dbg_flag & MP_DBG_NO_REFINE) || (opt->flag & MP_F_NO_ALIGN)) return false;
+	fprintf(stderr, "[miniprot_b200] --dbg-no-refine is supported with -A only (the reference aligns regions without refined anchors and crashes)\n");
+	return true;
+}
+
+void map_batch(Stages *st, const mp_idx_t *mi, const mp_mapopt_t *opt, const Batch &b, int32_t *n_reg_out, mp_reg1_t **reg_out, int32_t qr_tid)
 {
 	const int32_t n = b.n, kmer = mi->opt.kmer;
+	// one reading of the switches for the whole batch.  The entry points refuse --dbg-no-refine without -A (bad_dbg_flags); should
+	// that case get here anyway, the regions are refined as usual rather than aligned without anchors.
+	const int32_t dbg = mp_dbg_flag;
+	const bool qr = (dbg & MP_DBG_QNAME) && qr_tid >= 0, no_refine = (dbg & MP_DBG_NO_REFINE) && (opt->flag & MP_F_NO_ALIGN);
+	const bool dumps = qr || (dbg & (MP_DBG_ANCHOR | MP_DBG_CHAIN));
 	std::vector<QueryState> qs((size_t)n);
 	auto t_prev = std::chrono::steady_clock::now();
 	auto lap = [&](int phase) {
@@ -53,26 +103,37 @@ void map_batch(Stages *st, const mp_idx_t *mi, const mp_mapopt_t *opt, const Bat
 	// ---- S1
 	st->batch_begin(b);
 	ChainSet cs;
+	cs.want_seeds = (dbg & MP_DBG_ANCHOR) != 0;
 	st->seed_chain(mi, opt, b, cs);
+	const bool x_lines = cs.want_seeds && cs.seed_off.size() == (size_t)n + 1;
+	if (cs.want_seeds && !x_lines && n > 0) { // a backend that does not keep the seeding contract: no X lines rather than a bad read
+		static std::atomic<bool> warned{false};
+		if (!warned.exchange(true)) fprintf(stderr, "[WARNING] the seeding stage returned no seeds: --dbg-anchor prints nothing\n");
+	}
 	lap(0);
 
 	// ---- H1 + S2 work list
 	// (the host phases are independent per protein: contiguous ranges of proteins on the worker pool, per-range results
-	// concatenated in order)
+	// concatenated in order; so are the dump lines of the --dbg-* switches, formatted per range and written in order)
 	std::vector<RefineJob> rjobs;
 	std::vector<int32_t> rjob_first((size_t)n + 1, 0);
 	{
 		std::vector<std::vector<RefineJob>> part(64);
+		std::vector<Str> dump(dumps ? 64 : 0);
 		const int n_part = par_ranges(n, 64, [&](int lo, int hi, int c) {
 			std::vector<RefineJob> &out = part[(size_t)c];
 			for (int32_t q = lo; q < hi; ++q) {
 				QueryState &Q = qs[(size_t)q];
 				const int32_t n_u = (int32_t)(cs.u_off[(size_t)q + 1] - cs.u_off[(size_t)q]);
 				const uint64_t *u = cs.u.data() + cs.u_off[(size_t)q], *a = cs.a.data() + cs.a_off[(size_t)q];
+				if (qr) put_fmt(dump[(size_t)c], "QR\t%s\t%d\t%d\n", b.name && b.name[q] ? b.name[q] : "*", b.len[q], qr_tid); // map.c:268
+				if (x_lines) dump_seeds(dump[(size_t)c], mi, cs.seed_off[(size_t)q + 1] - cs.seed_off[(size_t)q], cs.seed.data() + cs.seed_off[(size_t)q]);
 				Q.reg = regs_from_chains(mi, n_u, u, a, &Q.n_reg);
 				regs_sort(&Q.n_reg, Q.reg);
 				regs_set_parent(opt->mask_level, opt->mask_len, Q.n_reg, Q.reg, kmer, 0);
 				regs_select_sub(opt->pri_ratio * opt->pri_ratio, kmer * 2, opt->best_n, &Q.n_reg, Q.reg);
+				if (dbg & MP_DBG_CHAIN) dump_chains(dump[(size_t)c], mi, Q.n_reg, Q.reg, a);
+				if (no_refine) continue;
 				regs_max_ext(0, Q.n_reg, Q.reg, a, 100, opt->max_ext, Q.ext);
 				for (int32_t i = 0; i < Q.n_reg; ++i) { // window of map.c:41-42
 					const mp_reg1_t *r = &Q.reg[i];
@@ -88,18 +149,26 @@ void map_batch(Stages *st, const mp_idx_t *mi, const mp_mapopt_t *opt, const Bat
 		});
 		for (int c = 0; c < n_part; ++c) rjobs.insert(rjobs.end(), part[(size_t)c].begin(), part[(size_t)c].end());
 		for (int32_t q = 0; q < n; ++q) rjob_first[(size_t)q + 1] = rjob_first[(size_t)q] + qs[(size_t)q].n_reg;
+		if (dumps) { // one block per batch: the dumps of contexts that map other units concurrently do not interleave with it
+			flockfile(stderr);
+			for (int c = 0; c < n_part; ++c) {
+				if (dump[(size_t)c].l) fwrite(dump[(size_t)c].s, 1, (size_t)dump[(size_t)c].l, stderr);
+				free(dump[(size_t)c].s);
+			}
+			funlockfile(stderr);
+		}
 	}
 	cs = ChainSet(); // first-round anchors are not needed any more
 	lap(1);
 
-	// ---- S2
+	// ---- S2 (none with --dbg-no-refine -A: the first-round regions are the result, map.c:205)
 	RefineSet rs;
-	st->refine(mi, opt, b, rjobs, rs);
+	if (!no_refine) st->refine(mi, opt, b, rjobs, rs);
 	lap(2);
 
 	// ---- H2: adopt refined chains (map.c:83-109), re-rank (map.c:217-221)
 	const int32_t k2 = opt->kmer2;
-	par_ranges(n, 64, [&](int q_lo, int q_hi, int) {
+	if (!no_refine) par_ranges(n, 64, [&](int q_lo, int q_hi, int) {
 	for (int32_t q = q_lo; q < q_hi; ++q) {
 		QueryState &Q = qs[(size_t)q];
 		int32_t kept = 0;
@@ -148,7 +217,8 @@ void map_batch(Stages *st, const mp_idx_t *mi, const mp_mapopt_t *opt, const Bat
 					regs_max_ext(mi->nt, Q.n_reg, Q.reg, Q.anchors.data(), 100, opt->max_intron / 2, Q.ext);
 					for (int32_t i = 0; i < Q.n_reg; ++i) {
 						RegionPlan p;
-						if (p.plan(mi, opt, q, b.len[q], b.seq[q], &Q.reg[i], (int32_t)(Q.ext[(size_t)i] >> 32), (int32_t)Q.ext[(size_t)i], pjobs[(size_t)c]))
+						if (p.plan(mi, opt, q, b.len[q], b.seq[q], &Q.reg[i], (int32_t)(Q.ext[(size_t)i] >> 32), (int32_t)Q.ext[(size_t)i], (dbg & MP_DBG_MORE_DP) != 0,
+						           pjobs[(size_t)c]))
 							pplan[(size_t)c].push_back(std::move(p));
 					}
 				}
@@ -326,12 +396,13 @@ private:
 // steps one after another on the calling thread for any input (A/B, debugging).
 int32_t map_file(Stages *st, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, FILE *out)
 {
+	if (bad_dbg_flags(opt)) return -3;
 	FastxReader rd(fn);
 	if (!rd.fp) return -1;
 	int64_t id_counter = 0;
 	if (opt->flag & MP_F_GFF) fputs("##gff-version 3\n", out); // map.c:338
 	auto map_step = [&](FileBatch &fb) {
-		map_batch(st, mi, opt, fb.view(), fb.n_reg.data(), fb.reg.data());
+		map_batch(st, mi, opt, fb.view(), fb.n_reg.data(), fb.reg.data(), 0);
 		if (mp_verbose >= 3)
 			fprintf(stderr, "[M::%s::%.3f*%.2f] mapped %d sequences\n", "map_file", mp_realtime(), mp_cputime() / mp_realtime(), (int)fb.seqs.size());
 	};
@@ -385,6 +456,7 @@ int32_t map_file_multi(Stages *const *st, int n, const mp_idx_t *mi, const char 
 {
 	if (n < 1) return -1;
 	if (n == 1) return map_file(st[0], mi, fn, opt, out);
+	if (bad_dbg_flags(opt)) return -3;
 	FastxReader rd(fn);
 	if (!rd.fp) return -1;
 	if (opt->flag & MP_F_GFF) fputs("##gff-version 3\n", out); // map.c:338
@@ -428,7 +500,7 @@ int32_t map_file_multi(Stages *const *st, int n, const mp_idx_t *mi, const char 
 					todo.pop_front();
 				}
 				FileBatch &fb = *u.second;
-				map_batch(st[k], mi, opt, fb.view(), fb.n_reg.data(), fb.reg.data());
+				map_batch(st[k], mi, opt, fb.view(), fb.n_reg.data(), fb.reg.data(), k);
 				if (mp_verbose >= 3)
 					fprintf(stderr, "[M::%s::%.3f*%.2f] mapped %d sequences (context %d)\n", "map_file_multi", mp_realtime(), mp_cputime() / mp_realtime(), (int)fb.seqs.size(), k);
 				std::lock_guard<std::mutex> lk(mu);

@@ -1,7 +1,8 @@
 """Differential fuzzing of the HOST side of the product under arbitrary command lines, on the CPU (no GPU needed): the reference's
 UNMODIFIED main.c linked against tests/_build/libhostcheck.so (the product's host sources -- options, index builder, .mpi I/O, hit
 bookkeeping, alignment planner, statistics, all output formats -- with the C oracle as stage backend) against the reference binary
-oracle/_ref/miniprot, same random options, same random synthetic inputs; stdout must be byte-identical.
+oracle/_ref/miniprot, same random options, same random synthetic inputs; stdout must be byte-identical, and so must the dump lines
+of the --dbg-* switches on stderr.
 Needs /root/reference (to compile main.c) and oracle/_ref.  Test infrastructure, not part of the product.
 
 usage: python tools/fuzz_cli.py [seed] [n_iterations] [workdir]"""
@@ -16,6 +17,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 import build_hostcheck  # noqa: E402
+import build_hostcheck_dbg  # noqa: E402
+import dbg_lib  # noqa: E402
 from miniprot_b200 import synth  # noqa: E402
 
 REF_SRC = os.environ.get("MPB_REFERENCE", "/root/reference")
@@ -148,6 +151,13 @@ def random_options(rng, g, d):
         o.extend(["--spsc", sp])
         maybe(0.3, "--spsc0", int(rng.integers(0, 15)))
         maybe(0.3, "--spsc-max", int(rng.integers(0, 15)))
+    # the debugging switches (mp_dbg_flag).  The dump lines go to stderr protein after protein only with one worker thread in the
+    # reference; --dbg-no-refine without -A crashes the reference (and is refused here), so those runs are skipped below
+    for sw, pr in (("--dbg-qname", 0.1), ("--dbg-anchor", 0.1), ("--dbg-chain", 0.1), ("--dbg-aflt", 0.15), ("--dbg-no-refine", 0.05), ("--no-kalloc", 0.05)):
+        if rng.random() < pr:
+            o.append(sw)
+    if any(x in o for x in ("--dbg-qname", "--dbg-anchor", "--dbg-chain")):
+        o[1] = "1"
     if rng.random() < float(os.environ.get("MPB_FUZZ_P_INDEX", 0.08)):  # index options (host index builder; the default index is what the GPU stages are built for)
         maybe(0.5, "-M", int(rng.choice([0, 2])))
         maybe(0.5, "-L", int(rng.choice([10, 50])))
@@ -162,6 +172,9 @@ def fuzz(seed, n_it, workdir=None):
     if cli is None or not os.path.exists(REF_BIN):
         print("needs the reference sources (main.c) and oracle/_ref/miniprot")
         return 0, 0
+    # the oracle backend that also returns the seeds (--dbg-anchor) stands in for the one the program is linked with: its mp_map_file
+    # and every symbol of the host pipeline come first
+    env_cli = dict(os.environ, LD_PRELOAD=build_hostcheck_dbg.build())
     rng = np.random.default_rng(seed)
     bad = n_ref_abort = 0
     with tempfile.TemporaryDirectory(dir=workdir) as d:
@@ -182,12 +195,16 @@ def fuzz(seed, n_it, workdir=None):
                 for k, binary in enumerate((REF_BIN, cli)):
                     subprocess.run([binary, "-t2", "-d", mpi[k]] + idx_opts + [g], check=True, stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
             for k, binary in enumerate((REF_BIN, cli)):
-                r = subprocess.run([binary] + opts + [mpi[1 - k] if use_mpi else g, p], stdout=subprocess.PIPE, stderr=subprocess.PIPE)
+                r = subprocess.run([binary] + opts + [mpi[1 - k] if use_mpi else g, p], stdout=subprocess.PIPE, stderr=subprocess.PIPE,
+                                   env=env_cli if k else None)
                 outs.append((r.returncode, r.stdout, r.stderr))
             if outs[0][0] < 0:  # the reference itself stopped at one of its assertions (e.g. align.c:200 with a tiny -J): nothing to compare with
                 n_ref_abort += 1
                 continue
-            same = outs[0][0] == outs[1][0] and outs[0][1] == outs[1][1]
+            if "--dbg-no-refine" in opts and "-A" not in opts:
+                n_ref_abort += 1
+                continue
+            same = outs[0][0] == outs[1][0] and outs[0][1] == outs[1][1] and dbg_lib.dump_lines(outs[0][2]) == dbg_lib.dump_lines(outs[1][2])
             same = same and b"Sanitizer" not in outs[1][2] and b"runtime error" not in outs[1][2]
             if use_mpi:
                 same = same and open(os.path.join(d, "i0.mpi"), "rb").read() == open(os.path.join(d, "i1.mpi"), "rb").read()
