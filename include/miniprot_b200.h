@@ -235,7 +235,8 @@ int mpb_idx_share(mpb_ctx_t *dst, mpb_ctx_t *src);
  * result cannot be reproduced bit for bit: a gap open penalty below 1 (with -O 0 the reference's lazy-F loop stops at once,
  * nasw-sse.c:411,530, and its scores depend on the SSE stripe layout) or an ie_coef whose length penalty has more steps
  * than the kernels' table (> ~5); or an index built with a minimum ORF length (-L) above 40, which the tile halos of the
- * window kernels do not cover.  mpb_map_file() and mpb_nasw_batch() apply the same checks. */
+ * window kernels do not cover.  mpb_map_file() and mpb_nasw_batch() apply the same checks, and mpb_refine_batch() the
+ * index check. */
 int mpb_map_batch(mpb_ctx_t *ctx, const mp_idx_t *mi, const mp_mapopt_t *opt, int32_t n_seq,
                   const char *const *seqs, const int32_t *lens, const char *const *names,
                   int32_t *n_reg_out, mp_reg1_t **reg_out);
@@ -292,7 +293,8 @@ int mpb_seed_batch(mpb_ctx_t *ctx, const mp_idx_t *mi, int32_t max_occ, int32_t 
 
 /* Second-round refinement over a batch of windows (replaces map.c:41-97 per region): window k is [as, ae) on strand
  * vid = contig<<1|rev of query qid.  On return a_off[n_win+1] / *a hold the best chain of each window
- * (window-relative nt end position<<32 | residue end position; empty = no chain) and sc[n_win] its score; *a is malloc'ed. */
+ * (window-relative nt end position<<32 | residue end position; empty = no chain) and sc[n_win] its score; *a is malloc'ed.
+ * Returns 0; -1 for a bad argument; -3 (with a message on stderr) for an index with a minimum ORF length above 40. */
 typedef struct { int32_t qid; uint32_t vid; int64_t as, ae; } mpb_window_t;
 int mpb_refine_batch(mpb_ctx_t *ctx, const mp_idx_t *mi, const mp_mapopt_t *opt, int32_t n_seq, const char *const *seqs, const int32_t *lens,
                      int32_t n_win, const mpb_window_t *win, int64_t *a_off, uint64_t **a, int32_t *sc);

@@ -419,7 +419,7 @@ def refine_batch(ctx: Context, mi, mo, seqs, windows):
     rc = L.mpb_refine_batch(ctx.h, C.cast(mi, C.c_void_p), C.cast(C.pointer(mo), C.c_void_p), n, C.cast(arr, C.c_void_p), lens.ctypes.data, nw,
                             C.cast(win, C.c_void_p), off.ctypes.data, C.byref(ap), sc.ctypes.data)
     if rc != 0:
-        raise RuntimeError("mpb_refine_batch failed")
+        raise RuntimeError(f"mpb_refine_batch failed ({rc})")
     a = np.ctypeslib.as_array(C.cast(ap, C.POINTER(C.c_uint64)), shape=(max(int(off[nw]), 1),)).copy()[:int(off[nw])]
     L.mpb_free(ap)
     return [(a[off[k]:off[k + 1]], int(sc[k])) for k in range(nw)]

@@ -823,6 +823,7 @@ int mpb_refine_batch(mpb_ctx_t *c, const mp_idx_t *mi, const mp_mapopt_t *opt, i
                      const mpb_window_t *win, int64_t *a_off, uint64_t **a, int32_t *sc)
 {
 	if (c == 0 || mi == 0 || opt == 0 || n_seq < 0 || n_win < 0) return -1;
+	if (bad_index(mi)) return -3;
 	std::lock_guard<std::mutex> cl(c->mu);
 	MPB_CUDA_OK(cudaSetDevice(c->device));
 	Batch b;

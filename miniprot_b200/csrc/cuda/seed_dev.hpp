@@ -10,8 +10,11 @@ namespace cuda {
 
 constexpr int SEED_THREADS = 128;
 constexpr int WIN_TILE = 2048;                 // window positions per shared-memory tile
-constexpr int WIN_SMEM_SPAN = WIN_TILE + 256;  // + halos of 3*(min_aa_len+1) on the left, 3*min_aa_len on the right
+constexpr int WIN_SMEM_SPAN = WIN_TILE + 256;  // + halos of 3*(max(min_aa_len,kmer)+1) on the left, 3*min_aa_len on the right
 constexpr int WIN_MAX_MIN_AA = 40;             // largest min_aa_len the halos cover
+constexpr int WIN_MAX_KMER = 7;                // largest k-mer (index -k, refinement -l): 4 bits a residue in a 32-bit word
+static_assert(WIN_MAX_KMER <= WIN_MAX_MIN_AA && 3 * (WIN_MAX_MIN_AA + 1) + 3 * WIN_MAX_MIN_AA <= WIN_SMEM_SPAN - WIN_TILE,
+              "the tile halos must fit in the shared-memory span for every min_aa_len <= WIN_MAX_MIN_AA and kmer <= WIN_MAX_KMER");
 
 struct SeedConst {          // passed by value (constant bank)
 	uint8_t aa13[256];      // residue char -> 4-bit reduced alphabet (>= 14: stop / unknown)

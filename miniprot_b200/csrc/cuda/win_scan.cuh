@@ -82,7 +82,9 @@ __device__ void scan_window(const uint8_t *packed, const WinJob &job, const Seed
 {
 	__shared__ uint32_t ok[3][WIN_WORDS];
 	const int64_t L = job.len;
-	const int halo_l = 3 * (min_aa_len + 1), halo_r = 3 * min_aa_len;
+	// the left halo covers the look-back of both run tests: min_aa_len codons for the ORF, kmer codons for the k-mer (the
+	// refinement's kmer2 may exceed min_aa_len)
+	const int halo_l = 3 * ((min_aa_len > kmer ? min_aa_len : kmer) + 1), halo_r = 3 * min_aa_len;
 	const uint32_t mask = (1u << kmer * 4) - 1;
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
 	for (int64_t t0 = pos_lo; t0 < L && t0 < pos_hi; t0 += WIN_TILE) {
@@ -107,7 +109,7 @@ __device__ void scan_window(const uint8_t *packed, const WinJob &job, const Seed
 		if (warp < 3) {
 			const uint32_t g = lane < WIN_WORDS ? ok[warp][lane] : 0;
 			const uint32_t in_orf = bits_spread_down(bits_run_ends(g, min_aa_len, lane), min_aa_len, lane);
-			const uint32_t v = min_aa_len >= kmer ? in_orf & bits_run_ends(g, kmer, lane) : 0;
+			const uint32_t v = in_orf & bits_run_ends(g, kmer, lane);  // an ORF shorter than kmer has no k-mer end
 			if (lane < WIN_WORDS) ok[warp][lane] = v;
 		}
 		__syncthreads();

@@ -2,7 +2,8 @@
 reference's entry points: the oracle-backed host library of the CPU tests or libminiprot_b200.so.  Shared by test_host_dbg.py and
 test_gpu_dbg.py, and by tools/fuzz_cli.py for the dump lines.
 
-A child process parses the few options below as main.c does (main.c:120-201), loads the index, sets mp_dbg_flag and calls
+A child process parses the few options below as main.c does (main.c:114-201; -k -M -L -b -l only in the attached form -k5),
+loads the index, sets mp_dbg_flag and calls
 mp_map_file: stdout is the PAF / GFF, stderr carries the dump lines, exactly where the reference CLI prints them."""
 import hashlib
 import json
@@ -26,6 +27,28 @@ _record = None
 SWITCH_SETS = [["--dbg-qname", "--dbg-anchor", "--dbg-chain"], ["--dbg-aflt"], ["--dbg-aflt", "--gff"], ["--dbg-aflt", "-j2"],
                ["--dbg-no-refine", "-A"], ["--dbg-qname", "--dbg-chain", "--dbg-no-refine", "-A"]]
 
+# index and refinement options off the defaults (-k 6 -M 1 -L 30 -b 8, -l 5), one CLI option list each: the k-mer masks and bucket
+# counts (-k, -M), the ORF rule and the window kernels' halos (-L; below -k the index is built on the host, below -l only the
+# refinement sees it), the block size (-b) and the refinement k-mer (-l).  4k <= 28 and -l <= 7 (a 32-bit k-mer word).
+INDEX_OPTION_SETS = [[], ["-k5"], ["-k4", "-M0"], ["-M0"], ["-M2"], ["-L6"], ["-L5"], ["-L1"], ["-L0"], ["-L4"], ["-L10"], ["-L40"],
+                     ["-b6"], ["-b7"], ["-b9"], ["-b10"], ["-l3"], ["-l4"], ["-l6"], ["-l7"], ["-l7", "-L5"], ["-l6", "-L4"],
+                     ["-l7", "-L1"], ["-k5", "-M0", "-L12", "-b9", "-l4"]]
+INDEX_SWITCHES = ["--dbg-anchor", "--dbg-chain"]  # the X (seeds) and Y1 (first-round chains) lines show which stage diverged
+_IDX_FIELD = {"-k": "kmer", "-M": "mod_bit", "-L": "min_aa_len", "-b": "bbit"}
+
+
+def index_options(opts) -> tuple:
+    """({IdxOpt field: value}, {MapOpt field: value}) of an option list of INDEX_OPTION_SETS (main.c:114-121)."""
+    io, mo = {}, {}
+    for a in opts:
+        if a[:2] in _IDX_FIELD:
+            io[_IDX_FIELD[a[:2]]] = int(a[2:])
+        elif a[:2] == "-l":
+            mo["kmer2"] = int(a[2:])
+        else:
+            raise ValueError(a)
+    return io, mo
+
 _CHILD = r"""
 import ctypes as C, os, sys
 sys.path.insert(0, sys.argv[1])
@@ -46,6 +69,8 @@ for i, a in enumerate(args):
     elif a.startswith("-j"): mo.sp_model = int(a[2:])
     elif a == "--spsc": spsc = args[i + 1]
     elif a.startswith("-K"): mo.mini_batch_size = int(a[2:])
+    elif a[:2] in ("-k", "-M", "-L", "-b"): setattr(io, {"-k": "kmer", "-M": "mod_bit", "-L": "min_aa_len", "-b": "bbit"}[a[:2]], int(a[2:]))
+    elif a[:2] == "-l": mo.kmer2 = int(a[2:])
 L.mp_idx_load.restype = C.c_void_p
 L.mp_idx_load.argtypes = [C.c_char_p, C.c_void_p, C.c_int32]
 mi = L.mp_idx_load(files[0].encode(), C.byref(io), 4)
@@ -175,5 +200,8 @@ if __name__ == "__main__":  # --record: the reference's answers for every case o
         ref_cli_dbg(["--dbg-qname", "--dbg-anchor", "--dbg-chain"], *sets["tiny"])
         ref_cli_dbg(["--dbg-aflt", "--spsc", spsc_file(d)], ol.DPP3_GENOME, ol.DPP3_PROTEIN)
         ref_cli_dbg(["--dbg-aflt"], *c4_slice(d))
+        for name in ("DPP3", "tiny", "tiny5"):  # test_host_index_options / test_gpu_index_options
+            for opts in INDEX_OPTION_SETS + [["-L41"]]:
+                ref_cli_dbg(opts + INDEX_SWITCHES, *sets[name])
     save_record()
     print(len(_record), "answers written to", RECORD_PATH)

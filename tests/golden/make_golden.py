@@ -9,7 +9,8 @@ expected outputs (SURVEY.md section 4), so these files ARE the golden vectors; m
 
 Then tests/golden/reference_calls.json.gz, every answer of the reference the tests compare with (tests/oracle_lib.py
 reference()): the CPU tests that ask it are run once against oracle/_ref/libref.so, and the reference CLI is run on the inputs
-of the GPU parity tests (test_gpu_e2e, test_gpu_dropin, test_gpu_configs; a few minutes for the 1 Gbp C3s shape).
+of the GPU parity tests (test_gpu_e2e, test_gpu_dropin, test_gpu_index_options, test_gpu_configs; a few minutes for the 1 Gbp
+C3s shape).
 """
 import os
 import subprocess
@@ -67,6 +68,11 @@ def answers(d):
     ol.ref_index_file(synth.generate(synth.CONFIGS["tiny"], os.path.join(d, "tiny"))[0])
     for g in (test_gpu_dropin.write_odd_fasta(os.path.join(d, "odd.fa")), ol.DPP3_GENOME, synth.generate(synth.CONFIGS["small"], os.path.join(d, "small"))[0]):
         ol.ref_index_file(g)
+    import test_gpu_index_options
+
+    for g in (test_gpu_dropin.write_odd_fasta(os.path.join(d, "odd.fa")), synth.generate(synth.CONFIGS["tiny"], os.path.join(d, "tiny"))[0]):
+        for opts in test_gpu_index_options.INDEX_SETS:
+            ol.ref_index_file(g, opts)
     for g, p in test_gpu_dropin.map_inputs(os.path.join(d, "tiny")):
         test_gpu_dropin.ref_regions(g, p)
     for g, p, _, args, _ in test_gpu_dropin.spsc_inputs(d):

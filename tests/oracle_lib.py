@@ -100,15 +100,15 @@ def ref_cli(args, genome: str, proteins: str | None = None, threads: int = 8) ->
     return reference(run, "cli", [file_digest(a) if os.path.isfile(a) else a for a in args], [file_digest(f) for f in files])
 
 
-def ref_index_file(genome: str) -> str:
-    """sha256 of the .mpi file the reference CLI writes for `genome` (-d)."""
+def ref_index_file(genome: str, args=()) -> str:
+    """sha256 of the .mpi file the reference CLI writes for `args -d FILE genome` (args: index options such as -k5 -L12)."""
     def run():
         import tempfile
         with tempfile.TemporaryDirectory() as d:
             out = os.path.join(d, "ref.mpi")
-            subprocess.run([REF_BIN, "-t4", "-d", out, genome], check=True, capture_output=True)
+            subprocess.run([REF_BIN, "-t4", *args, "-d", out, genome], check=True, capture_output=True)
             return file_digest(out)
-    return reference(run, "cli -d", file_digest(genome))
+    return reference(run, "cli -d", file_digest(genome), *([list(args)] if args else []))
 
 
 def build_oracle():
@@ -337,14 +337,16 @@ def random_dp_problem(rng: np.random.Generator, al_max=60, intron_max=400, p_sub
     return nt, aa.encode()
 
 
-def random_chain_problem(rng: np.random.Generator, n: int, mode: str):
-    """Sorted anchors for the three mp_chain call regimes: 'pre', 'main' (block ids) and 'refine' (base resolution)."""
+def random_chain_problem(rng: np.random.Generator, n: int, mode: str, bbit: int = 8):
+    """Sorted anchors for the three mp_chain call regimes: 'pre', 'main' (block ids of 1 << bbit bases) and 'refine' (base
+    resolution)."""
     if mode in ("pre", "main"):
         nb = max(4, n // 3)
         x = np.sort(rng.integers(1000, 1000 + nb, size=n)).astype(np.uint64)
         base = rng.integers(5, 400, size=n)
-        # plant collinear runs: qpos follows block id * 85 (256/3) within clusters
-        y = ((x.astype(np.int64) - 1000) * 85 % 380 + rng.integers(0, 40, size=n) + 5).astype(np.uint64)
+        # plant collinear runs: qpos follows block id * the residues of a block (85 = 256/3 at bbit 8) within clusters
+        f = max(1, (1 << bbit) // 3)
+        y = ((x.astype(np.int64) - 1000) * f % max(380, 4 * f + 40) + rng.integers(0, 40, size=n) + 5).astype(np.uint64)
         y = np.where(rng.random(n) < 0.3, base.astype(np.uint64), y)
     else:
         x = np.sort(rng.integers(14, 14 + 6 * n + 50, size=n)).astype(np.uint64)

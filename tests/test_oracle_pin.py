@@ -105,23 +105,36 @@ def test_sort128x_matches_reference_permutation():
             assert (np.diff(b[:, 0].astype(np.int64)) >= 0).all()
 
 
+class _V(C.Structure):  # mp64_v
+    _fields_ = [("n", C.c_int32), ("m", C.c_int32), ("a", C.POINTER(C.c_uint64))]
+
+
+def sketch_prot(seq, L, k, m):  # the reference's sketch, stored as its digest
+    v = _V()
+    ol.ref().ref_mp_sketch_prot(None, seq, L, k, m, C.byref(v))
+    return ol._digest(np.array([v.a[i] for i in range(v.n)], np.uint64))
+
+
+def sketch_nt4(nt, L, k, m, bbit, boff, min_aa_len=30):
+    v = _V()
+    ol.ref().ref_mp_sketch_nt4(None, nt.ctypes.data_as(C.c_void_p), C.c_int64(L), min_aa_len, k, m, bbit, C.c_int64(boff), C.byref(v))
+    return ol._digest(np.array([v.a[i] for i in range(v.n)], np.uint64))
+
+
+def orf_rich_genome(rng, L, n_rate=0.0):
+    """L random bases with most stop codons of frame 0 removed (long ORFs), N at rate n_rate."""
+    nt = rng.integers(0, 4, size=L).astype(np.uint8)
+    for s in range(0, L - 2, 3):
+        if nt[s] == 3 and ((nt[s + 1] == 0 and nt[s + 2] in (0, 2)) or (nt[s + 1] == 2 and nt[s + 2] == 0)):
+            nt[s] = 1
+    if n_rate:
+        nt[rng.random(L) < n_rate] = 4
+    return nt
+
+
 def test_hash_and_sketch(tab):
     rng = np.random.default_rng(3)
     o = ol.ora()
-
-    class V(C.Structure):
-        _fields_ = [("n", C.c_int32), ("m", C.c_int32), ("a", C.POINTER(C.c_uint64))]
-
-    def sketch_prot(seq, L, k, m):  # the reference's sketch, stored as its digest
-        v = V()
-        ol.ref().ref_mp_sketch_prot(None, seq, L, k, m, C.byref(v))
-        return ol._digest(np.array([v.a[i] for i in range(v.n)], np.uint64))
-
-    def sketch_nt4(nt, L, k, m, bbit, boff):
-        v = V()
-        ol.ref().ref_mp_sketch_nt4(None, nt.ctypes.data_as(C.c_void_p), C.c_int64(L), 30, k, m, bbit, C.c_int64(boff), C.byref(v))
-        return ol._digest(np.array([v.a[i] for i in range(v.n)], np.uint64))
-
     for it in range(40):
         L = int(rng.integers(1, 600))
         alpha = b"ARNDCQEGHILKMFPSTWYV" + (b"X*" if it % 3 == 0 else b"")
@@ -146,6 +159,44 @@ def test_hash_and_sketch(tab):
             n = o.ora_sketch_nt4(C.byref(tab), nt.ctypes.data_as(C.c_void_p), C.c_int64(L), 30, k, m, bbit, C.c_int64(boff),
                                  out.ctypes.data_as(C.c_void_p))
             assert ol._digest(out[:n]) == want, (it, k, n)
+
+
+@pytest.mark.parametrize("min_aa_len", [0, 1, 4, 5, 6, 29, 31, 40])
+def test_sketch_nt4_index_options(tab, min_aa_len):
+    """The genome sketch (index build, and with bbit 0 the refinement's window sketch) at -L below, at and above -k / -l, at the
+    defaults' neighbours and at the largest -L the window kernels take, for every -k 4..7, -M 0 / 2 and -b 0 / 9."""
+    rng = np.random.default_rng(500 + min_aa_len)
+    o = ol.ora()
+    genomes = [orf_rich_genome(rng, 3000), orf_rich_genome(rng, 800, 0.01), rng.integers(0, 4, size=200).astype(np.uint8)]
+    n_kmers = 0
+    for nt in genomes:
+        L = len(nt)
+        for k in (4, 5, 6, 7):
+            for m in (0, 2):
+                for bbit, boff in ((0, 0), (9, 77)):
+                    want = ol.reference(lambda: sketch_nt4(nt, L, k, m, bbit, boff, min_aa_len), "mp_sketch_nt4 -L", nt, min_aa_len, k, m, bbit, boff)
+                    out = np.zeros(L + 1, np.uint64)
+                    n = o.ora_sketch_nt4(C.byref(tab), nt.ctypes.data_as(C.c_void_p), C.c_int64(L), min_aa_len, k, m, bbit, C.c_int64(boff),
+                                         out.ctypes.data_as(C.c_void_p))
+                    assert ol._digest(out[:n]) == want, (L, k, m, bbit)
+                    n_kmers += n
+    assert n_kmers > 0
+
+
+@pytest.mark.parametrize("k", [3, 4, 5, 6, 7])
+def test_sketch_prot_kmer_sizes(tab, k):
+    """The protein sketch at every refinement k-mer size (-l 3..7; mod_bit 0) and index k-mer size with -M 2."""
+    rng = np.random.default_rng(600 + k)
+    o = ol.ora()
+    for it in range(20):
+        L = int(rng.integers(1, 400)) if it else k - 1  # one protein shorter than a k-mer
+        alpha = b"ARNDCQEGHILKMFPSTWYV" + (b"X*" if it % 3 == 0 else b"")
+        seq = bytes(alpha[i] for i in rng.integers(0, len(alpha), size=L))
+        for m in (0, 2):
+            want = ol.reference(lambda: sketch_prot(seq, L, k, m), "mp_sketch_prot", seq, k, m)
+            out = np.zeros(L + 1, np.uint64)
+            n = o.ora_sketch_prot(C.byref(tab), seq, L, k, m, out.ctypes.data_as(C.c_void_p))
+            assert ol._digest(out[:n]) == want, (it, L, m)
 
 
 @pytest.mark.parametrize("mode", ["pre", "main", "refine"])

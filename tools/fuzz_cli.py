@@ -158,7 +158,7 @@ def random_options(rng, g, d):
             o.append(sw)
     if any(x in o for x in ("--dbg-qname", "--dbg-anchor", "--dbg-chain")):
         o[1] = "1"
-    if rng.random() < float(os.environ.get("MPB_FUZZ_P_INDEX", 0.08)):  # index options (host index builder; the default index is what the GPU stages are built for)
+    if rng.random() < float(os.environ.get("MPB_FUZZ_P_INDEX", 0.08)):  # index options (host index builder; tests/test_gpu_index_options.py runs the GPU stages under them)
         maybe(0.5, "-M", int(rng.choice([0, 2])))
         maybe(0.5, "-L", int(rng.choice([10, 50])))
         maybe(0.3, "-b", int(rng.choice([7, 9])))
