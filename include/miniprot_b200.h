@@ -241,6 +241,23 @@ int mpb_map_batch(mpb_ctx_t *ctx, const mp_idx_t *mi, const mp_mapopt_t *opt, in
                   const char *const *seqs, const int32_t *lens, const char *const *names,
                   int32_t *n_reg_out, mp_reg1_t **reg_out);
 
+/* Locus mode: align proteins to genomic loci the caller already knows (lifting gene models over, re-aligning the hits of a
+ * translated search, checking annotated loci).  Pair k is protein seqs[loci[k].qid] against [st, en) of contig cid, both strands.
+ * reg_out[k] / n_reg_out[k] receive what the reference reports when that locus alone is the genome (its index built with mi->opt,
+ * the mapping options as given; -I is not applied, opt->max_intron is used as it is), secondary hits included, moved to the
+ * coordinates of the real genome: vid = cid<<1|rev, and vs / ve and every feat[].vs / ve gain st on the + strand, len(cid) - en
+ * on the - strand.  mpb_format_paf() with mi then prints the reference's PAF line for the locus, with the contig's name and
+ * length in columns 6-7 and start and end moved by st.  Free the regions with mpb_regs_free(n_loci, ...).
+ * mi needs its genome only (an index from mpb_idx_load_meta will do): the loci are seeded without a k-mer table.  A context that
+ * holds mi resident uploads nothing of it; otherwise only the packed genome and the contig table are uploaded.
+ * Returns 0; -1 (nothing mapped) for a null context or a malformed locus: qid or cid out of range, st < 0, en > len(cid) or
+ * st >= en; -3 (with a message, nothing mapped) for what mpb_map_batch() refuses, an index with --spsc scores, or any
+ * mp_dbg_flag bit other than MP_DBG_NO_KALLOC. */
+typedef struct { int32_t qid, cid; int64_t st, en; } mpb_locus_t;
+int mpb_map_loci(mpb_ctx_t *ctx, const mp_idx_t *mi, const mp_mapopt_t *opt, int32_t n_seq, const char *const *seqs,
+                 const int32_t *lens, const char *const *names, int32_t n_loci, const mpb_locus_t *loci,
+                 int32_t *n_reg_out, mp_reg1_t **reg_out);
+
 /* mp_map_file() with an explicit output stream and context (tests, benchmarks). */
 int32_t mpb_map_file(mpb_ctx_t *ctx, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, FILE *out);
 /* mpb_map_file() over n_ctx distinct contexts (on one or several GPUs) at once: the input is cut into units of at most
@@ -290,6 +307,13 @@ int mpb_chain_batch(mpb_ctx_t *ctx, const mpb_chain_par_t *par, int32_t n, const
  * On return a_off[n+1] / *a hold each query's sorted anchors (block<<32|qpos); *a is malloc'ed. */
 int mpb_seed_batch(mpb_ctx_t *ctx, const mp_idx_t *mi, int32_t max_occ, int32_t n_seq, const char *const *seqs,
                    const int32_t *lens, int64_t *a_off, uint64_t **a);
+
+/* The seeding of locus mode alone (mpb_map_loci): a_off[n_loci+1] / *a hold each pair's sorted, max_occ-filtered anchors
+ * (block<<32|qpos), the blocks numbered as in an index of the locus alone (the - strand's from ceil(len / 2^bbit)); *a is
+ * malloc'ed.  Returns 0; -1 as mpb_map_loci(); -3 (with a message) for an index mpb_map_batch() refuses, --spsc scores or
+ * debugging bits as mpb_map_loci(). */
+int mpb_seed_loci_batch(mpb_ctx_t *ctx, const mp_idx_t *mi, int32_t max_occ, int32_t n_seq, const char *const *seqs,
+                        const int32_t *lens, int32_t n_loci, const mpb_locus_t *loci, int64_t *a_off, uint64_t **a);
 
 /* Second-round refinement over a batch of windows (replaces map.c:41-97 per region): window k is [as, ae) on strand
  * vid = contig<<1|rev of query qid.  On return a_off[n_win+1] / *a hold the best chain of each window

@@ -397,6 +397,104 @@ def seed_batch(ctx: Context, mi, max_occ: int, seqs):
     return [a[off[i]:off[i + 1]] for i in range(n)]
 
 
+class Locus(C.Structure):  # mpb_locus_t
+    _fields_ = [("qid", C.c_int32), ("cid", C.c_int32), ("st", C.c_int64), ("en", C.c_int64)]
+
+
+def _loci_args(seqs, loci, names=None):
+    import numpy as np
+
+    n, nl = len(seqs), len(loci)
+    arr = (C.c_char_p * max(n, 1))(*seqs)
+    nam = (C.c_char_p * max(n, 1))(*(names or [b"*"] * n))
+    lens = np.array([len(s) for s in seqs] or [0], np.int32)
+    loc = (Locus * max(nl, 1))(*[Locus(*l) for l in loci])
+    return n, nl, arr, nam, lens, loc
+
+
+def map_loci(ctx: Context, mi, mo: MapOpt, seqs, names, loci, L: C.CDLL | None = None, fn: str = "mpb_map_loci"):
+    """mpb_map_loci: loci = list of (qid, cid, st, en).  Returns (rc, n_reg int32 array, reg array of mp_reg1_t pointers); free the
+    regions with free_loci_regs.  `L` / `fn`: another library exporting the same call without its context argument (the CPU tests'
+    oracle-backed hc_map_loci), ctx is then None."""
+    import numpy as np
+
+    n, nl, arr, nam, lens, loc = _loci_args(seqs, loci, names)
+    n_reg = np.zeros(max(nl, 1), np.int32)
+    reg = (C.c_void_p * max(nl, 1))()
+    f = getattr(L or lib(), fn)
+    f.restype = C.c_int
+    f.argtypes = ([C.c_void_p] if ctx is not None else []) + [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
+                                                              C.c_void_p, C.c_void_p]
+    args = [C.cast(mi, C.c_void_p), C.cast(C.pointer(mo), C.c_void_p), n, C.cast(arr, C.c_void_p), lens.ctypes.data, C.cast(nam, C.c_void_p), nl,
+            C.cast(loc, C.c_void_p), n_reg.ctypes.data, C.cast(reg, C.c_void_p)]
+    rc = f(*([ctx.h] if ctx is not None else []), *args)
+    return rc, n_reg[:nl], reg
+
+
+def free_loci_regs(n_reg, reg) -> None:
+    """What mpb_regs_free does, with the C library's free (the regions of either library are libc-allocated)."""
+    import ctypes.util
+
+    libc = C.CDLL(ctypes.util.find_library("c"))
+    libc.free.argtypes = [C.c_void_p]
+    for k in range(len(n_reg)):
+        if not reg[k]:
+            continue
+        rp = C.cast(reg[k], C.POINTER(Reg1))
+        for j in range(int(n_reg[k])):
+            libc.free(C.cast(rp[j].feat, C.c_void_p)), libc.free(C.cast(rp[j].p, C.c_void_p))
+        libc.free(reg[k])
+
+
+def loci_paf(mi, mo: MapOpt, seqs, names, loci, n_reg, reg, L: C.CDLL | None = None, fn: str = "mpb_format_paf") -> bytes:
+    """The PAF lines of map_loci's regions, pair by pair: the hits the reference's writer prints for a protein (map.c:293-326: the
+    first out_n, with a positive score of at least out_sim times the best and a query coverage of at least out_cov), formatted by
+    mpb_format_paf (or `fn` of `L`) with the real index."""
+    f = getattr(L or lib(), fn)
+    f.restype = C.c_int64
+    f.argtypes = [C.c_void_p, C.c_void_p, C.c_char_p, C.c_int32, C.c_char_p, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+    buf, ln, cap = C.c_void_p(), C.c_int64(0), C.c_int64(0)
+    for k, (qid, _, _, _) in enumerate(loci):
+        nr = int(n_reg[k])
+        if nr == 0:
+            continue
+        rp = C.cast(reg[k], C.POINTER(Reg1))
+        sc = lambda r: r.p.contents.dp_max if r.p else r.chn_sc  # noqa: E731
+        best = sc(rp[0])
+        for j in range(min(nr, mo.out_n)):
+            r = rp[j]
+            if sc(r) <= 0 or sc(r) < best * mo.out_sim or r.qe - r.qs < len(seqs[qid]) * mo.out_cov:
+                continue
+            f(C.cast(mi, C.c_void_p), C.cast(C.pointer(mo), C.c_void_p), names[qid], len(seqs[qid]), seqs[qid], C.addressof(r), C.byref(buf), C.byref(ln), C.byref(cap))
+    out = C.string_at(buf, ln.value) if ln.value else b""
+    if buf:
+        free = (L or lib()).mpb_free if L is None else C.CDLL(None).free
+        free.argtypes = [C.c_void_p]
+        free(buf)
+    return out
+
+
+def seed_loci_batch(ctx: Context, mi, max_occ: int, seqs, loci):
+    """mpb_seed_loci_batch: the sorted, max_occ-filtered anchors (block<<32 | qpos, blocks of an index of the locus alone) of every
+    (qid, cid, st, en) pair."""
+    import numpy as np
+
+    n, nl, arr, _, lens, loc = _loci_args(seqs, loci)
+    off = np.zeros(nl + 1, np.int64)
+    ap = C.c_void_p()
+    L = lib()
+    L.mpb_seed_loci_batch.restype = C.c_int
+    L.mpb_seed_loci_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
+                                      C.POINTER(C.c_void_p)]
+    rc = L.mpb_seed_loci_batch(ctx.h, C.cast(mi, C.c_void_p), max_occ, n, C.cast(arr, C.c_void_p), lens.ctypes.data, nl, C.cast(loc, C.c_void_p),
+                               off.ctypes.data, C.byref(ap))
+    if rc != 0:
+        raise RuntimeError(f"mpb_seed_loci_batch failed ({rc})")
+    a = np.ctypeslib.as_array(C.cast(ap, C.POINTER(C.c_uint64)), shape=(max(int(off[nl]), 1),)).copy()[:int(off[nl])]
+    L.mpb_free(ap)
+    return [a[off[k]:off[k + 1]] for k in range(nl)]
+
+
 class Window(C.Structure):  # mpb_window_t
     _fields_ = [("qid", C.c_int32), ("vid", C.c_uint32), ("as_", C.c_int64), ("ae", C.c_int64)]
 

@@ -83,15 +83,27 @@ void build_spsc_table(mpb_ctx_s *c, const mp_idx_t *mi)
 }
 
 int acquire_index(mpb_ctx_s *c, const mp_idx_t *mi);
+int acquire_genome(mpb_ctx_s *c, const mp_idx_t *mi);
 void pin_to_device_node(int device);
 
 struct CudaStages : Stages {
 	mpb_ctx_s *ctx;
 	explicit CudaStages(mpb_ctx_s *c) : ctx(c) {}
 
+	// locus mode (loci_view): the stages called with `view` read the resident genome of `view_of`; the k-mer tables are not needed
+	const mp_idx_t *view = 0, *view_of = 0;
+	bool loci_view(const mp_idx_t *mi, const mp_idx_t *v) override
+	{
+		view_of = mi, view = v;
+		return true;
+	}
 	void need_index(const mp_idx_t *mi)
 	{
-		if (ctx->mi != mi || !ctx->d_seq) {
+		if (mi && mi == view) {
+			if (acquire_genome(ctx, view_of) != 0) { fprintf(stderr, "[miniprot_b200] genome upload failed\n"); abort(); }
+			return;
+		}
+		if (ctx->mi != mi || !ctx->d_seq || !ctx->d_ki) {
 			if (acquire_index(ctx, mi) != 0) { fprintf(stderr, "[miniprot_b200] index upload failed\n"); abort(); }
 		}
 	}
@@ -136,6 +148,13 @@ struct CudaStages : Stages {
 		std::vector<int32_t> off;
 		const char *d_aa = upload_residues(b, off);
 		seed_chain_run(ctx, mi, opt, b, off, d_aa, out);
+	}
+	void seed_chain_loci(const mp_idx_t *vi, const mp_mapopt_t *opt, const Batch &b, ChainSet &out) override
+	{
+		need_index(vi);
+		std::vector<int32_t> off;
+		const char *d_aa = upload_residues(b, off);
+		seed_chain_loci_run(ctx, vi, opt, b, off, d_aa, out);
 	}
 	void refine(const mp_idx_t *mi, const mp_mapopt_t *opt, const Batch &b, const std::vector<RefineJob> &jobs, RefineSet &out) override
 	{
@@ -368,7 +387,7 @@ int idx_share_unlocked(mpb_ctx_s *dst, mpb_ctx_s *src)
 int acquire_index(mpb_ctx_s *c, const mp_idx_t *mi)
 {
 	std::lock_guard<std::mutex> il(g_idx_mu);
-	if (c->mi == mi && c->d_seq) return 0;
+	if (c->mi == mi && c->d_seq && c->d_ki) return 0;
 	mpb_ctx_s *src = 0;
 	{
 		std::lock_guard<std::mutex> lk(g_default_mu);
@@ -376,6 +395,26 @@ int acquire_index(mpb_ctx_s *c, const mp_idx_t *mi)
 			if (o != c && o->mi == mi && o->d_ki && o->d_kb && o->d_seq && (!src || (o->device == c->device && src->device != c->device))) src = o;
 	}
 	return src ? idx_share_unlocked(c, src) : idx_upload_unlocked(c, mi);
+}
+
+// CudaStages::need_index in locus mode: mi's genome resident in c.  Nothing is uploaded when c holds mi (with or without its k-mer
+// tables); otherwise only the packed genome and the contig table are, never the k-mer tables (mi may have none: mpb_idx_load_meta).
+int acquire_genome(mpb_ctx_s *c, const mp_idx_t *mi)
+{
+	std::lock_guard<std::mutex> il(g_idx_mu);
+	if (c->mi == mi && c->d_seq) return 0;
+	if (!mi || !mi->nt || !mi->nt->seq) return -1;
+	MPB_CUDA_OK(cudaSetDevice(c->device));
+	forget_adopters(c);
+	forget_index(c);
+	const size_t seq_bytes = (size_t)((mi->nt->l_seq + 1) >> 1);
+	c->own_seq.reserve(seq_bytes + 16);
+	MPB_CUDA_OK(cudaMemcpy(c->own_seq.p, mi->nt->seq, seq_bytes, cudaMemcpyHostToDevice));
+	c->d_seq = c->own_seq.as<uint8_t>();
+	upload_meta(c, mi);
+	c->mi = mi, c->own_index = true;
+	c->stats.h2d_bytes += (int64_t)seq_bytes;
+	return 0;
 }
 
 // MPB_DEVICES=<device>[,<device>...] (repeats allowed: "0,0" = two contexts on device 0), read once; empty when unset
@@ -649,6 +688,52 @@ int mpb_map_batch(mpb_ctx_t *c, const mp_idx_t *mi, const mp_mapopt_t *opt, int3
 	return map_batch_on(c, mi, opt, n_seq, seqs, lens, names, n_reg_out, reg_out, 0);
 }
 
+int mpb_map_loci(mpb_ctx_t *c, const mp_idx_t *mi, const mp_mapopt_t *opt, int32_t n_seq, const char *const *seqs, const int32_t *lens,
+                 const char *const *names, int32_t n_loci, const mpb_locus_t *loci, int32_t *n_reg_out, mp_reg1_t **reg_out)
+{
+	if (!c || !opt) return -1;
+	const int rc = check_loci(mi, n_seq, n_loci, loci);
+	if (rc != 0) return rc;
+	if (bad_scoring(opt->go, opt->ie_coef) || bad_index(mi)) return -3;
+	std::lock_guard<std::mutex> cl(c->mu);
+	MPB_CUDA_OK(cudaSetDevice(c->device));
+	return map_loci(c->stages, mi, opt, n_seq, seqs, lens, names, n_loci, loci, n_reg_out, reg_out);
+}
+
+int mpb_seed_loci_batch(mpb_ctx_t *c, const mp_idx_t *mi, int32_t max_occ, int32_t n_seq, const char *const *seqs, const int32_t *lens, int32_t n_loci,
+                        const mpb_locus_t *loci, int64_t *a_off, uint64_t **a)
+{
+	if (!c) return -1;
+	const int rc = check_loci(mi, n_seq, n_loci, loci);
+	if (rc != 0) return rc;
+	if (bad_index(mi)) return -3;
+	std::lock_guard<std::mutex> cl(c->mu);
+	MPB_CUDA_OK(cudaSetDevice(c->device));
+	LocusView v(mi, n_loci, loci);
+	std::vector<const char*> sp((size_t)n_loci);
+	std::vector<int32_t> lp((size_t)n_loci);
+	for (int32_t k = 0; k < n_loci; ++k) sp[(size_t)k] = seqs[loci[k].qid], lp[(size_t)k] = lens[loci[k].qid];
+	Batch b;
+	b.n = n_loci, b.seq = sp.data(), b.len = lp.data(), b.name = 0;
+	std::vector<int64_t> ao((size_t)n_loci + 1, 0);
+	std::vector<uint64_t> av;
+	if (n_loci > 0) {
+		CudaStages *cs = static_cast<CudaStages*>(c->stages);
+		cs->loci_view(mi, &v.idx);
+		cs->need_index(&v.idx);
+		std::vector<int32_t> off;
+		const char *d_aa = cs->upload_residues(b, off);
+		seed_loci_batch_run(c, &v.idx, max_occ, b, off, d_aa, ao, av);
+		cs->loci_view(0, 0);
+	}
+	for (int32_t k = 0; k <= n_loci; ++k) a_off[k] = ao[(size_t)k];
+	for (int32_t k = 0; k < n_loci; ++k) // view block ids -> those of an index of the locus alone
+		for (int64_t j = ao[(size_t)k]; j < ao[(size_t)k + 1]; ++j) av[(size_t)j] -= (uint64_t)v.bo[(size_t)k * 2] << 32;
+	*a = (uint64_t*)malloc(sizeof(uint64_t) * (av.size() + 1));
+	if (!av.empty()) memcpy(*a, av.data(), sizeof(uint64_t) * av.size());
+	return 0;
+}
+
 int32_t mpb_map_file(mpb_ctx_t *c, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, FILE *out)
 {
 	if (!c) return -1;
@@ -680,7 +765,7 @@ int32_t mpb_map_file_multi(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_idx_t 
 	// the index is resident in every context before the mappers start: in the first one that holds it or can upload it, shared
 	// from there to the others (on the same device nothing is copied)
 	for (int32_t k = 0; k < n_ctx; ++k) {
-		if (ctx[k]->mi == mi && ctx[k]->d_seq) continue;
+		if (ctx[k]->mi == mi && ctx[k]->d_seq && ctx[k]->d_ki) continue;
 		if (acquire_index(ctx[k], mi) != 0) { fprintf(stderr, "[miniprot_b200] the index is neither resident in a context nor on the host\n"); return -1; }
 	}
 	std::vector<Stages*> st((size_t)n_ctx);

@@ -58,6 +58,35 @@ __device__ int64_t block_kth(const int64_t *cnt, int n, int64_t k, int64_t vmax,
 	return lo;
 }
 
+// map.c:158-167 over the bucket sizes cnt[0..n) (all <= vmax) of one protein's seeds: the adaptive occupancy cut-off (map.c:126-141),
+// then the exclusive scan of the sizes that pass it into aoff[] (-1 marks a dropped bucket).  Returns the number of anchors.
+__device__ __forceinline__ int64_t occ_cut_scan(const int64_t *cnt, int n, int32_t max_occ, int64_t vmax, int64_t *aoff, int64_t *red, int64_t &scan_carry)
+{
+	if (n >= 8) { // map.c:158-161 + 126-141
+		const int64_t q25 = block_kth(cnt, n, (int64_t)(n * .25 + .499), vmax, red);
+		const int64_t q75 = block_kth(cnt, n, (int64_t)(n * .75 + .499), vmax, red);
+		const int32_t cap = (int32_t)((double)(uint64_t)q75 + (double)(uint64_t)(q75 - q25) * 1.5 + 10.);
+		if (cap < max_occ) max_occ = cap;
+	}
+	// exclusive scan of the effective bucket sizes (0 for buckets above the cap)
+	if (threadIdx.x == 0) scan_carry = 0;
+	__syncthreads();
+	for (int i0 = 0; i0 < n; i0 += blockDim.x) {
+		const int i = i0 + threadIdx.x;
+		int64_t v = (i < n && cnt[i] <= max_occ) ? cnt[i] : 0, inc = v;
+		for (int d = 1; d < 32; d <<= 1) { const int64_t o = __shfl_up_sync(0xffffffffu, inc, d); if ((int)(threadIdx.x & 31) >= d) inc += o; }
+		if ((threadIdx.x & 31) == 31) red[threadIdx.x >> 5] = inc;
+		__syncthreads();
+		int64_t wbase = scan_carry;
+		for (int w = 0; w < (int)(threadIdx.x >> 5); ++w) wbase += red[w];
+		if (i < n) aoff[i] = cnt[i] <= max_occ ? wbase + inc - v : -1;
+		__syncthreads();
+		if (threadIdx.x == blockDim.x - 1) scan_carry = wbase + inc;
+		__syncthreads();
+	}
+	return scan_carry;
+}
+
 __global__ void __launch_bounds__(SEED_THREADS) seed_sketch_kernel(const char *aa, const int32_t *aa_off, int n_q, SeedConst cst, const int64_t *ki,
                                                                    uint32_t *sd_hash, int32_t *sd_pos, int64_t *sd_cnt, int64_t *sd_aoff,
                                                                    int32_t *n_sd_out, int64_t *tot_out)
@@ -84,31 +113,8 @@ __global__ void __launch_bounds__(SEED_THREADS) seed_sketch_kernel(const char *a
 	}
 	__syncthreads();
 	const int n = n_sd_s;
-	int64_t *cnt = sd_cnt + base;
-	int32_t max_occ = cst.max_occ;
-	if (n >= 8) { // map.c:158-161 + 126-141
-		const int64_t q25 = block_kth(cnt, n, (int64_t)(n * .25 + .499), cst.n_kb, red);
-		const int64_t q75 = block_kth(cnt, n, (int64_t)(n * .75 + .499), cst.n_kb, red);
-		const int32_t cap = (int32_t)((double)(uint64_t)q75 + (double)(uint64_t)(q75 - q25) * 1.5 + 10.);
-		if (cap < max_occ) max_occ = cap;
-	}
-	// exclusive scan of the effective bucket sizes (0 for buckets above the cap)
-	if (threadIdx.x == 0) scan_carry = 0;
-	__syncthreads();
-	for (int i0 = 0; i0 < n; i0 += blockDim.x) {
-		const int i = i0 + threadIdx.x;
-		int64_t v = (i < n && cnt[i] <= max_occ) ? cnt[i] : 0, inc = v;
-		for (int d = 1; d < 32; d <<= 1) { const int64_t o = __shfl_up_sync(0xffffffffu, inc, d); if ((int)(threadIdx.x & 31) >= d) inc += o; }
-		if ((threadIdx.x & 31) == 31) red[threadIdx.x >> 5] = inc;
-		__syncthreads();
-		int64_t wbase = scan_carry;
-		for (int w = 0; w < (int)(threadIdx.x >> 5); ++w) wbase += red[w];
-		if (i < n) sd_aoff[base + i] = cnt[i] <= max_occ ? wbase + inc - v : -1; // -1 marks a dropped bucket
-		__syncthreads();
-		if (threadIdx.x == blockDim.x - 1) scan_carry = wbase + inc;
-		__syncthreads();
-	}
-	if (threadIdx.x == 0) n_sd_out[q] = n, tot_out[q] = scan_carry;
+	const int64_t tot = occ_cut_scan(sd_cnt + base, n, cst.max_occ, cst.n_kb, sd_aoff + base, red, scan_carry);
+	if (threadIdx.x == 0) n_sd_out[q] = n, tot_out[q] = tot;
 }
 
 __global__ void __launch_bounds__(SEED_THREADS) seed_expand_kernel(const int32_t *aa_off, int n_q, const int64_t *ki, const uint32_t *kb, const uint32_t *sd_hash,
@@ -129,8 +135,10 @@ __global__ void __launch_bounds__(SEED_THREADS) seed_expand_kernel(const int32_t
 	}
 }
 
-// all k-mers (mod 0) of every protein: key = hash<<32 | pos, written at aa_off[q] + slot; n_out[q] = count
-__global__ void __launch_bounds__(SEED_THREADS) prot_kmer_kernel(const char *aa, const int32_t *aa_off, int n_q, SeedConst cst, int kmer, uint64_t *keys, int32_t *n_out)
+// the k-mers of every protein whose hash passes the mod filter (sketch.c:18; mod_bit 0: all of them): key = hash>>mod_bit<<32 | pos,
+// written at aa_off[q] + slot; n_out[q] = count
+__global__ void __launch_bounds__(SEED_THREADS) prot_kmer_kernel(const char *aa, const int32_t *aa_off, int n_q, SeedConst cst, int kmer, int mod_bit, uint64_t *keys,
+                                                                 int32_t *n_out)
 {
 	__shared__ int n_s;
 	const int q = blockIdx.x;
@@ -138,12 +146,14 @@ __global__ void __launch_bounds__(SEED_THREADS) prot_kmer_kernel(const char *aa,
 	const int32_t base = aa_off[q], L = aa_off[q + 1] - base;
 	if (threadIdx.x == 0) n_s = 0;
 	__syncthreads();
-	const uint32_t mask = (1u << kmer * 4) - 1;
+	const uint32_t mask = (1u << kmer * 4) - 1, mod = (1u << mod_bit) - 1;
 	for (int i = threadIdx.x; i < L; i += blockDim.x) {
 		uint32_t x;
 		if (!prot_kmer_at(aa + base, i, kmer, cst, x)) continue;
+		const uint32_t h = hash32_mask_dev(x, mask);
+		if (h & mod) continue;
 		const int slot = atomicAdd(&n_s, 1);
-		keys[base + slot] = (uint64_t)hash32_mask_dev(x, mask) << 32 | (uint32_t)i;
+		keys[base + slot] = (uint64_t)(h >> mod_bit) << 32 | (uint32_t)i;
 	}
 	__syncthreads();
 	if (threadIdx.x == 0) n_out[q] = n_s;
@@ -220,6 +230,107 @@ __global__ void __launch_bounds__(SEED_THREADS) win_emit_kernel(const WinJob *jo
 	});
 }
 
+// ---- locus seeding: what the reference seeds from an index of one locus, without a k-mer table -----------------------------
+// The ORF scan of the index build runs over both strands of the locus; a k-mer is kept when its bucket is one of the protein's
+// seed buckets (binary search in the protein's sorted seeds).  Count pass, then emit pass: bucket<<32 | block, the block numbered
+// from the strand's first block boff.  Ranges of tiles of one strand per CTA, as in the index build.
+template <bool EMIT>
+__global__ void __launch_bounds__(SEED_THREADS) locus_join_kernel(const LocusUnit *units, const LocusStrand *strands, const uint8_t *packed, SeedConst cst, int min_aa_len,
+                                                                  int bbit, const uint64_t *pk_all, const int32_t *aa_off, const int32_t *n_pk, const int64_t *unit_off,
+                                                                  int64_t *unit_n, uint64_t *out)
+{
+	extern __shared__ uint8_t sm[];
+	__shared__ unsigned long long n_s;
+	const LocusUnit u = units[blockIdx.x];
+	const LocusStrand s = strands[u.strand];
+	const uint64_t *pk = pk_all + aa_off[s.qid];
+	const int npk = n_pk[s.qid];
+	if (npk == 0) { // nothing to join with
+		if (!EMIT && threadIdx.x == 0) unit_n[blockIdx.x] = 0;
+		return;
+	}
+	if (threadIdx.x == 0) n_s = 0;
+	__syncthreads();
+	WinJob job;
+	job.g_start = s.g_start, job.dir = s.dir, job.comp = s.comp, job.len = s.len, job.qid = s.qid, job.pad_ = 0, job.grp_off = 0;
+	const uint32_t mod = (1u << cst.mod_bit) - 1;
+	uint64_t *o = EMIT ? out + unit_off[blockIdx.x] : 0;
+	scan_window(packed, job, cst, cst.kmer, min_aa_len, sm, sm + WIN_SMEM_SPAN, [&](uint32_t h, int64_t e) {
+		if (h & mod) return;
+		const uint32_t b = h >> cst.mod_bit;
+		const int lo = lower_hash(pk, npk, b);
+		if (lo >= npk || (uint32_t)(pk[lo] >> 32) != b) return;
+		const unsigned long long k = atomicAdd(&n_s, 1ULL);
+		if (EMIT) o[k] = (uint64_t)b << 32 | (uint32_t)((e >> bbit) + s.boff); // sketch.c:58: block of the codon's last base
+	}, u.pos_lo, u.pos_hi);
+	if (!EMIT && threadIdx.x == 0) unit_n[blockIdx.x] = (int64_t)n_s; // (scan_window ends with a barrier)
+}
+
+// the distinct keys of each sorted segment keys[seg[q], seg[q+1]) -- a locus's (bucket, block) pairs, what index.c:71-90 holds for
+// it -- to the same place in blk (their block halves only) and uniq (whole keys); n_u[q] = how many.  One CTA per segment.
+__global__ void __launch_bounds__(SEED_THREADS) locus_unique_kernel(const uint64_t *keys, const int64_t *seg, int n_q, uint64_t *uniq, uint32_t *blk, int64_t *n_u)
+{
+	__shared__ int64_t red[SEED_THREADS / 32];
+	__shared__ int64_t carry;
+	const int q = blockIdx.x;
+	if (q >= n_q) return;
+	const int64_t b = seg[q], n = seg[q + 1] - b;
+	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+	if (threadIdx.x == 0) carry = 0;
+	__syncthreads();
+	for (int64_t i0 = 0; i0 < n; i0 += blockDim.x) {
+		const int64_t i = i0 + threadIdx.x;
+		const bool first = i < n && (i == 0 || keys[b + i] != keys[b + i - 1]);
+		const uint32_t m = __ballot_sync(0xffffffffu, first);
+		if (lane == 0) red[warp] = __popc(m);
+		__syncthreads();
+		int64_t base = carry, tot = 0;
+		for (int w = 0; w < (int)(blockDim.x >> 5); ++w) { if (w < warp) base += red[w]; tot += red[w]; }
+		if (first) {
+			const int64_t k = b + base + __popc(m & ((1u << lane) - 1));
+			uniq[k] = keys[b + i], blk[k] = (uint32_t)keys[b + i];
+		}
+		__syncthreads();
+		if (threadIdx.x == 0) carry += tot;
+		__syncthreads();
+	}
+	if (threadIdx.x == 0) n_u[q] = carry;
+}
+
+// first index in the sorted keys u[0..n) that is >= x
+__device__ __forceinline__ int64_t lower_u64(const uint64_t *u, int64_t n, uint64_t x)
+{
+	int64_t lo = 0, hi = n;
+	while (lo < hi) { const int64_t mid = (lo + hi) >> 1; if (u[mid] < x) lo = mid + 1; else hi = mid; }
+	return lo;
+}
+
+// per protein (one CTA): the size of each seed's bucket in the locus's distinct pairs and where it starts, the adaptive occupancy
+// cut-off and the anchor offsets (occ_cut_scan, as seed_sketch_kernel does with the k-mer table), and the per-seed inputs of
+// seed_expand_kernel: its "ki" is sd_lo indexed by sd_idx (the seed's own slot), its "kb" the block halves of the distinct pairs
+__global__ void __launch_bounds__(SEED_THREADS) locus_occ_kernel(const uint64_t *pk_all, const int32_t *aa_off, const int32_t *n_pk, int n_q, const uint64_t *uniq,
+                                                                 const int64_t *seg, const int64_t *n_u, int32_t max_occ, uint32_t *sd_idx, int32_t *sd_pos,
+                                                                 int64_t *sd_lo, int64_t *sd_cnt, int64_t *sd_aoff, int64_t *tot_out)
+{
+	__shared__ int64_t red[SEED_THREADS / 32];
+	__shared__ int64_t scan_carry;
+	const int q = blockIdx.x;
+	if (q >= n_q) return;
+	const int32_t base = aa_off[q];
+	const int n = n_pk[q];
+	const uint64_t *u = uniq + seg[q];
+	const int64_t nu = n_u[q];
+	for (int i = threadIdx.x; i < n; i += blockDim.x) {
+		const uint64_t key = pk_all[base + i], b = key >> 32;
+		const int64_t lo = lower_u64(u, nu, b << 32), hi = lower_u64(u, nu, (b + 1) << 32);
+		sd_idx[base + i] = (uint32_t)(base + i), sd_pos[base + i] = (int32_t)(uint32_t)key;
+		sd_lo[base + i] = seg[q] + lo, sd_cnt[base + i] = hi - lo;
+	}
+	__syncthreads();
+	const int64_t tot = occ_cut_scan(sd_cnt + base, n, max_occ, nu, sd_aoff + base, red, scan_carry);
+	if (threadIdx.x == 0) tot_out[q] = tot;
+}
+
 // ---- launchers ----------------------------------------------------------------------------------------------
 void seed_launch_sketch(cudaStream_t st, const char *aa, const int32_t *aa_off, int n_q, const SeedConst &cst, const int64_t *ki, uint32_t *sd_hash, int32_t *sd_pos,
                         int64_t *sd_cnt, int64_t *sd_aoff, int32_t *n_sd, int64_t *tot)
@@ -231,9 +342,25 @@ void seed_launch_expand(cudaStream_t st, const int32_t *aa_off, int n_q, const i
 {
 	if (n_q > 0) seed_expand_kernel<<<n_q, SEED_THREADS, 0, st>>>(aa_off, n_q, ki, kb, sd_hash, sd_pos, sd_cnt, sd_aoff, n_sd, a_off, a);
 }
-void seed_launch_prot_kmer(cudaStream_t st, const char *aa, const int32_t *aa_off, int n_q, const SeedConst &cst, int kmer, uint64_t *keys, int32_t *n_out)
+void seed_launch_prot_kmer(cudaStream_t st, const char *aa, const int32_t *aa_off, int n_q, const SeedConst &cst, int kmer, int mod_bit, uint64_t *keys, int32_t *n_out)
 {
-	if (n_q > 0) prot_kmer_kernel<<<n_q, SEED_THREADS, 0, st>>>(aa, aa_off, n_q, cst, kmer, keys, n_out);
+	if (n_q > 0) prot_kmer_kernel<<<n_q, SEED_THREADS, 0, st>>>(aa, aa_off, n_q, cst, kmer, mod_bit, keys, n_out);
+}
+void locus_launch_join(cudaStream_t st, bool emit, const LocusUnit *units, int n_units, const LocusStrand *strands, const uint8_t *packed, const SeedConst &cst,
+                       int min_aa_len, int bbit, const uint64_t *pk, const int32_t *aa_off, const int32_t *n_pk, const int64_t *unit_off, int64_t *unit_n, uint64_t *out)
+{
+	if (n_units <= 0) return;
+	if (emit) locus_join_kernel<true><<<n_units, SEED_THREADS, 2 * WIN_SMEM_SPAN, st>>>(units, strands, packed, cst, min_aa_len, bbit, pk, aa_off, n_pk, unit_off, unit_n, out);
+	else locus_join_kernel<false><<<n_units, SEED_THREADS, 2 * WIN_SMEM_SPAN, st>>>(units, strands, packed, cst, min_aa_len, bbit, pk, aa_off, n_pk, unit_off, unit_n, out);
+}
+void locus_launch_unique(cudaStream_t st, const uint64_t *keys, const int64_t *seg, int n_q, uint64_t *uniq, uint32_t *blk, int64_t *n_u)
+{
+	if (n_q > 0) locus_unique_kernel<<<n_q, SEED_THREADS, 0, st>>>(keys, seg, n_q, uniq, blk, n_u);
+}
+void locus_launch_occ(cudaStream_t st, const uint64_t *pk, const int32_t *aa_off, const int32_t *n_pk, int n_q, const uint64_t *uniq, const int64_t *seg, const int64_t *n_u,
+                      int32_t max_occ, uint32_t *sd_idx, int32_t *sd_pos, int64_t *sd_lo, int64_t *sd_cnt, int64_t *sd_aoff, int64_t *tot)
+{
+	if (n_q > 0) locus_occ_kernel<<<n_q, SEED_THREADS, 0, st>>>(pk, aa_off, n_pk, n_q, uniq, seg, n_u, max_occ, sd_idx, sd_pos, sd_lo, sd_cnt, sd_aoff, tot);
 }
 void win_launch_count(cudaStream_t st, const WinJob *jobs, int n_jobs, const uint8_t *packed, const SeedConst &cst, int kmer, int min_aa_len, int max_ava,
                       const uint64_t *pk, const int32_t *aa_off, const int32_t *n_pk, int32_t *grp, int64_t *n_a)

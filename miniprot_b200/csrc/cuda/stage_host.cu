@@ -231,6 +231,18 @@ void seed_batch_run(mpb_ctx_s *ctx, const mp_idx_t *mi, int32_t max_occ, const B
 	ctx->stats.d2h_bytes += (int64_t)(sizeof(uint64_t) * a.size());
 }
 
+// map.c:186-195: pre-chain and main chain of every query's sorted seeds (d_a at a_off)
+static void chain_seeds(mpb_ctx_s *ctx, const mp_idx_t *mi, const mp_mapopt_t *opt, int n_q, const std::vector<int64_t> &a_off, const int64_t *d_a_off, uint64_t *d_a,
+                        ChainSet &out)
+{
+	const int32_t w = 1 << mi->opt.bbit, spl = !(opt->flag & MP_F_NO_SPLICE);
+	const chn::Par pre = chain_par(w, w, w, opt, 2, 0, mi->opt.kmer, mi->opt.bbit);
+	const chn::Par mainp = chain_par(opt->max_intron, opt->max_gap, opt->bw, opt, opt->min_chn_cnt, opt->min_chn_sc, mi->opt.kmer, mi->opt.bbit);
+	std::vector<int32_t> n_u, n_b;
+	chain_problems(ctx, n_q, a_off, d_a_off, d_a, (!(opt->flag & MP_F_NO_PRE_CHAIN) && spl) ? &pre : 0, mainp, n_u, n_b, out.u, out.a);
+	for (int q = 0; q < n_q; ++q) out.u_off[(size_t)q + 1] = out.u_off[(size_t)q] + n_u[(size_t)q], out.a_off[(size_t)q + 1] = out.a_off[(size_t)q] + n_b[(size_t)q];
+}
+
 void seed_chain_run(mpb_ctx_s *ctx, const mp_idx_t *mi, const mp_mapopt_t *opt, const Batch &b, const std::vector<int32_t> &aa_off, const char *d_aa, ChainSet &out)
 {
 	const int n_q = b.n;
@@ -247,12 +259,133 @@ void seed_chain_run(mpb_ctx_s *ctx, const mp_idx_t *mi, const mp_mapopt_t *opt, 
 		MPB_CUDA_OK(cudaStreamSynchronize(ctx->stream));
 		ctx->stats.d2h_bytes += (int64_t)(sizeof(uint64_t) * out.seed.size());
 	}
-	const int32_t w = 1 << mi->opt.bbit, spl = !(opt->flag & MP_F_NO_SPLICE);
-	const chn::Par pre = chain_par(w, w, w, opt, 2, 0, mi->opt.kmer, mi->opt.bbit);
-	const chn::Par mainp = chain_par(opt->max_intron, opt->max_gap, opt->bw, opt, opt->min_chn_cnt, opt->min_chn_sc, mi->opt.kmer, mi->opt.bbit);
-	std::vector<int32_t> n_u, n_b;
-	chain_problems(ctx, n_q, a_off, d_a_off, d_a, (!(opt->flag & MP_F_NO_PRE_CHAIN) && spl) ? &pre : 0, mainp, n_u, n_b, out.u, out.a);
-	for (int q = 0; q < n_q; ++q) out.u_off[(size_t)q + 1] = out.u_off[(size_t)q] + n_u[(size_t)q], out.a_off[(size_t)q + 1] = out.a_off[(size_t)q] + n_b[(size_t)q];
+	chain_seeds(ctx, mi, opt, n_q, a_off, d_a_off, d_a, out);
+}
+
+// Seeding of a batch of loci (map_loci): query q against contig q of the locus view vi only, exactly what the reference seeds from an
+// index of that locus alone.  There is no k-mer table; per batch:
+//   protein seeds (prot_kmer_kernel with the mod filter) -> sort per protein -> ORF scan of both strands of every locus, keeping the
+//   k-mers whose bucket the protein has (count, [D2H], emit) -> sort + unique per locus: its (bucket, block) pairs, as index.c:71-90
+//   holds them -> bucket sizes, adaptive occupancy cut-off, anchor offsets [D2H] -> seed_expand_kernel -> sort per query.
+// On return a_off[n_q + 1] delimits each query's sorted anchors (view block ids) inside *d_a_out (ctx->b_c[1]).
+static void seed_loci_run(mpb_ctx_s *ctx, const mp_idx_t *vi, int32_t max_occ, const Batch &b, const std::vector<int32_t> &aa_off, const char *d_aa,
+                          std::vector<int64_t> &a_off, uint64_t **d_a_out, int64_t **d_off_out)
+{
+	cudaStream_t st = ctx->stream;
+	const int n_q = b.n;
+	const size_t R = (size_t)aa_off[(size_t)n_q];
+	SeedConst cst;
+	mp_mapopt_t tmp;
+	memset(&tmp, 0, sizeof(tmp));
+	tmp.max_occ = max_occ;
+	fill_seed_const(vi, &tmp, cst);
+	std::vector<LocusStrand> strands((size_t)n_q * 2);
+	std::vector<LocusUnit> units;
+	std::vector<size_t> unit_first((size_t)n_q + 1, 0);
+	for (int q = 0; q < n_q; ++q) {
+		const mp_ctg_t *c = &vi->nt->ctg[q];
+		for (int s = 0; s < 2; ++s) {
+			LocusStrand &ls = strands[(size_t)q * 2 + s];
+			ls.g_start = s ? c->off + c->len - 1 : c->off, ls.dir = s ? -1 : 1, ls.comp = s, ls.len = c->len, ls.boff = vi->bo[q * 2 + s], ls.qid = q;
+			const int64_t step = (int64_t)WIN_TILE * 16;
+			for (int64_t p = 0; p < c->len; p += step) units.push_back(LocusUnit{ q * 2 + s, 0, p, std::min(p + step, (int64_t)c->len) });
+		}
+		unit_first[(size_t)q + 1] = units.size();
+	}
+	const int n_units = (int)units.size();
+	int32_t *d_aa_off, *d_npk, *sd_pos;
+	uint32_t *sd_idx;
+	uint64_t *d_pk, *d_pk_tmp;
+	int64_t *sd_lo, *sd_cnt, *sd_aoff, *d_unit_off, *d_unit_n, *d_seg, *d_nu, *d_tot, *d_a_off;
+	LocusUnit *d_units;
+	LocusStrand *d_strands;
+	auto layout = [&](Carver &c) {
+		d_aa_off = c.take<int32_t>((size_t)n_q + 1), d_npk = c.take<int32_t>((size_t)n_q), d_pk = c.take<uint64_t>(R + 1), d_pk_tmp = c.take<uint64_t>(R + 1);
+		sd_idx = c.take<uint32_t>(R + 1), sd_pos = c.take<int32_t>(R + 1), sd_lo = c.take<int64_t>(R + 1), sd_cnt = c.take<int64_t>(R + 1), sd_aoff = c.take<int64_t>(R + 1);
+		d_units = c.take<LocusUnit>((size_t)n_units + 1), d_strands = c.take<LocusStrand>(strands.size());
+		d_unit_off = c.take<int64_t>((size_t)n_units + 1), d_unit_n = c.take<int64_t>((size_t)n_units + 1);
+		d_seg = c.take<int64_t>((size_t)n_q + 1), d_nu = c.take<int64_t>((size_t)n_q), d_tot = c.take<int64_t>((size_t)n_q), d_a_off = c.take<int64_t>((size_t)n_q + 1);
+	};
+	ctx->b_c[0].reserve(carve_size(layout));
+	Carver cv(ctx->b_c[0].p);
+	layout(cv);
+	MPB_CUDA_OK(cudaMemcpyAsync(d_aa_off, aa_off.data(), sizeof(int32_t) * ((size_t)n_q + 1), cudaMemcpyHostToDevice, st));
+	if (n_units) MPB_CUDA_OK(cudaMemcpyAsync(d_units, units.data(), sizeof(LocusUnit) * units.size(), cudaMemcpyHostToDevice, st));
+	MPB_CUDA_OK(cudaMemcpyAsync(d_strands, strands.data(), sizeof(LocusStrand) * strands.size(), cudaMemcpyHostToDevice, st));
+	ctx->stats.h2d_bytes += (int64_t)(sizeof(LocusUnit) * units.size() + sizeof(LocusStrand) * strands.size());
+	ctx->time_begin();
+	// protein seeds, sorted per protein
+	seed_launch_prot_kmer(st, d_aa, d_aa_off, n_q, cst, cst.kmer, cst.mod_bit, d_pk, d_npk);
+	std::vector<int32_t> n_pk((size_t)n_q);
+	MPB_CUDA_OK(cudaMemcpyAsync(n_pk.data(), d_npk, sizeof(int32_t) * (size_t)n_q, cudaMemcpyDeviceToHost, st));
+	MPB_CUDA_OK(cudaStreamSynchronize(st));
+	{
+		std::vector<int64_t> sb((size_t)n_q), se((size_t)n_q);
+		for (int q = 0; q < n_q; ++q) sb[(size_t)q] = aa_off[(size_t)q], se[(size_t)q] = aa_off[(size_t)q] + n_pk[(size_t)q];
+		seg_sort_u64(ctx, st, d_pk, d_pk_tmp, n_q, sb.data(), se.data());
+	}
+	// the join: count, then emit at per-unit offsets
+	locus_launch_join(st, false, d_units, n_units, d_strands, ctx->d_seq, cst, vi->opt.min_aa_len, vi->opt.bbit, d_pk, d_aa_off, d_npk, 0, d_unit_n, 0);
+	std::vector<int64_t> unit_n((size_t)n_units + 1, 0), unit_off((size_t)n_units + 1, 0), seg((size_t)n_q + 1, 0);
+	if (n_units) MPB_CUDA_OK(cudaMemcpyAsync(unit_n.data(), d_unit_n, sizeof(int64_t) * (size_t)n_units, cudaMemcpyDeviceToHost, st));
+	MPB_CUDA_OK(cudaStreamSynchronize(st));
+	for (int u = 0; u < n_units; ++u) unit_off[(size_t)u + 1] = unit_off[(size_t)u] + unit_n[(size_t)u];
+	for (int q = 0; q <= n_q; ++q) seg[(size_t)q] = unit_off[unit_first[(size_t)q]];
+	const size_t M = (size_t)seg[(size_t)n_q];
+	MPB_CUDA_OK(cudaMemcpyAsync(d_unit_off, unit_off.data(), sizeof(int64_t) * unit_off.size(), cudaMemcpyHostToDevice, st));
+	MPB_CUDA_OK(cudaMemcpyAsync(d_seg, seg.data(), sizeof(int64_t) * seg.size(), cudaMemcpyHostToDevice, st));
+	ctx->b_c[4].reserve(sizeof(uint64_t) * (M + 2)), ctx->b_c[5].reserve(sizeof(uint64_t) * (M + 2)), ctx->b_c[6].reserve(sizeof(uint32_t) * (M + 2));
+	uint64_t *d_pairs = ctx->b_c[4].as<uint64_t>(), *d_uniq = ctx->b_c[5].as<uint64_t>();
+	uint32_t *d_blk = ctx->b_c[6].as<uint32_t>();
+	locus_launch_join(st, true, d_units, n_units, d_strands, ctx->d_seq, cst, vi->opt.min_aa_len, vi->opt.bbit, d_pk, d_aa_off, d_npk, d_unit_off, 0, d_pairs);
+	seg_sort_u64(ctx, st, d_pairs, d_uniq, n_q, seg.data(), seg.data() + 1);
+	locus_launch_unique(st, d_pairs, d_seg, n_q, d_uniq, d_blk, d_nu);
+	// bucket sizes, occupancy cut-off, expansion
+	locus_launch_occ(st, d_pk, d_aa_off, d_npk, n_q, d_uniq, d_seg, d_nu, max_occ, sd_idx, sd_pos, sd_lo, sd_cnt, sd_aoff, d_tot);
+	std::vector<int64_t> tot((size_t)n_q);
+	a_off.assign((size_t)n_q + 1, 0);
+	MPB_CUDA_OK(cudaMemcpyAsync(tot.data(), d_tot, sizeof(int64_t) * (size_t)n_q, cudaMemcpyDeviceToHost, st));
+	MPB_CUDA_OK(cudaStreamSynchronize(st));
+	for (int q = 0; q < n_q; ++q) a_off[(size_t)q + 1] = a_off[(size_t)q] + tot[(size_t)q];
+	const size_t N = (size_t)a_off[(size_t)n_q];
+	MPB_CUDA_OK(cudaMemcpyAsync(d_a_off, a_off.data(), sizeof(int64_t) * a_off.size(), cudaMemcpyHostToDevice, st));
+	ctx->b_c[1].reserve(sizeof(uint64_t) * (N + 2));
+	ctx->b_c[2].reserve(sizeof(uint64_t) * (N + 2));
+	uint64_t *d_a = ctx->b_c[1].as<uint64_t>(), *d_tmp = ctx->b_c[2].as<uint64_t>();
+	seed_launch_expand(st, d_aa_off, n_q, sd_lo, d_blk, sd_idx, sd_pos, sd_cnt, sd_aoff, d_npk, d_a_off, d_a);
+	seg_sort_u64(ctx, st, d_a, d_tmp, n_q, a_off.data(), a_off.data() + 1);
+	ctx->stats.ms_seed += ctx->time_end();
+	MPB_CUDA_OK(cudaGetLastError());
+	ctx->stats.kernel_launches += 6;
+	ctx->stats.n_anchors += (int64_t)N;
+	*d_a_out = d_a, *d_off_out = d_a_off;
+}
+
+void seed_chain_loci_run(mpb_ctx_s *ctx, const mp_idx_t *vi, const mp_mapopt_t *opt, const Batch &b, const std::vector<int32_t> &aa_off, const char *d_aa, ChainSet &out)
+{
+	const int n_q = b.n;
+	out.u_off.assign((size_t)n_q + 1, 0), out.a_off.assign((size_t)n_q + 1, 0), out.u.clear(), out.a.clear();
+	if (n_q == 0) return;
+	std::vector<int64_t> a_off;
+	uint64_t *d_a = 0;
+	int64_t *d_a_off = 0;
+	seed_loci_run(ctx, vi, opt->max_occ, b, aa_off, d_aa, a_off, &d_a, &d_a_off);
+	chain_seeds(ctx, vi, opt, n_q, a_off, d_a_off, d_a, out);
+}
+
+// stage-level entry for tests: locus seeding only (mpb_seed_loci_batch)
+void seed_loci_batch_run(mpb_ctx_s *ctx, const mp_idx_t *vi, int32_t max_occ, const Batch &b, const std::vector<int32_t> &aa_off, const char *d_aa,
+                         std::vector<int64_t> &a_off, std::vector<uint64_t> &a)
+{
+	uint64_t *d_a = 0;
+	int64_t *d_off = 0;
+	a_off.assign((size_t)b.n + 1, 0), a.clear();
+	if (b.n == 0) return;
+	seed_loci_run(ctx, vi, max_occ, b, aa_off, d_aa, a_off, &d_a, &d_off);
+	a.resize((size_t)a_off[(size_t)b.n]);
+	if (!a.empty()) MPB_CUDA_OK(cudaMemcpyAsync(a.data(), d_a, sizeof(uint64_t) * a.size(), cudaMemcpyDeviceToHost, ctx->stream));
+	MPB_CUDA_OK(cudaStreamSynchronize(ctx->stream));
+	ctx->stats.d2h_bytes += (int64_t)(sizeof(uint64_t) * a.size());
 }
 
 void refine_run(mpb_ctx_s *ctx, const mp_idx_t *mi, const mp_mapopt_t *opt, const Batch &b, const std::vector<int32_t> &aa_off, const char *d_aa,
@@ -287,7 +420,7 @@ void refine_run(mpb_ctx_s *ctx, const mp_idx_t *mi, const mp_mapopt_t *opt, cons
 	layout(cv);
 	MPB_CUDA_OK(cudaMemcpyAsync(d_aa_off, aa_off.data(), sizeof(int32_t) * ((size_t)n_q + 1), cudaMemcpyHostToDevice, st));
 	ctx->time_begin();
-	seed_launch_prot_kmer(st, d_aa, d_aa_off, n_q, cst, k2, d_pk, d_npk);
+	seed_launch_prot_kmer(st, d_aa, d_aa_off, n_q, cst, k2, 0, d_pk, d_npk);
 	MPB_CUDA_OK(cudaMemcpyAsync(n_pk.data(), d_npk, sizeof(int32_t) * (size_t)n_q, cudaMemcpyDeviceToHost, st));
 	MPB_CUDA_OK(cudaStreamSynchronize(st));
 	for (int q = 0; q < n_q; ++q) seg_b[(size_t)q] = aa_off[(size_t)q], seg_e[(size_t)q] = aa_off[(size_t)q] + n_pk[(size_t)q];

@@ -13,6 +13,12 @@ void seed_chain_run(mpb_ctx_s *ctx, const mp_idx_t *mi, const mp_mapopt_t *opt, 
 void refine_run(mpb_ctx_s *ctx, const mp_idx_t *mi, const mp_mapopt_t *opt, const Batch &b, const std::vector<int32_t> &aa_off, const char *d_aa,
                 const std::vector<RefineJob> &jobs, RefineSet &out);
 
+// S1 of locus mode (map_loci): query q seeded against contig q of the locus view vi alone, without a k-mer table; then the same chains
+void seed_chain_loci_run(mpb_ctx_s *ctx, const mp_idx_t *vi, const mp_mapopt_t *opt, const Batch &b, const std::vector<int32_t> &aa_off, const char *d_aa,
+                         ChainSet &out);
+void seed_loci_batch_run(mpb_ctx_s *ctx, const mp_idx_t *vi, int32_t max_occ, const Batch &b, const std::vector<int32_t> &aa_off, const char *d_aa,
+                         std::vector<int64_t> &a_off, std::vector<uint64_t> &a);
+
 void seed_batch_run(mpb_ctx_s *ctx, const mp_idx_t *mi, int32_t max_occ, const Batch &b, const std::vector<int32_t> &aa_off, const char *d_aa,
                     std::vector<int64_t> &a_off, std::vector<uint64_t> &a);
 void chain_batch_run(mpb_ctx_s *ctx, const chn::Par &par, int n_prob, const int64_t *a_off, const uint64_t *a, std::vector<int32_t> &n_u, std::vector<int32_t> &n_b,

@@ -112,7 +112,34 @@ struct Stages {
 	// called on a host thread before it first calls the stages (the mapper threads of map_file_multi): a device backend makes its
 	// device current there and keeps the thread on the device's NUMA node; optional
 	virtual void thread_init() {}
+	// Locus mode (map_loci).  loci_view(mi, view): until loci_view(0, 0), the stages called with `view` -- an index whose contigs are
+	// slices of mi's genome and that has no k-mer tables (LocusView) -- read mi's genome.  False: the backend has no locus mode.
+	virtual bool loci_view(const mp_idx_t * /*mi*/, const mp_idx_t * /*view*/) { return false; }
+	// S1 of locus mode: query q is seeded against contig q of `view` alone, as the reference seeds from an index of that locus
+	// (index.c:52-136 over a one-record FASTA), then chained as in seed_chain
+	virtual void seed_chain_loci(const mp_idx_t * /*view*/, const mp_mapopt_t * /*opt*/, const Batch & /*b*/, ChainSet & /*out*/) {}
 };
+
+// ---------------------------------------------------------------- locus mode (pipeline.cpp)
+// The index of one batch of loci: contig q is the locus of pair q, a view into mi's packed genome (nothing is copied), with block ids
+// numbered over these contigs as index.c:11-26 numbers a genome's; ki / kb stay null.  Contig names are the real contigs'.
+struct LocusView {
+	mp_idx_t idx;
+	mp_ntdb_t nt;
+	std::vector<mp_ctg_t> ctg;
+	std::vector<uint32_t> bo;
+	LocusView(const mp_idx_t *mi, int32_t n, const mpb_locus_t *loci);
+	LocusView(const LocusView &) = delete;
+	LocusView &operator=(const LocusView &) = delete;
+};
+// -1 for a malformed locus (qid or cid out of range, st < 0, en > contig length, st >= en); -3 with a message for what locus mode
+// refuses (--spsc scores, any mp_dbg_flag bit but MP_DBG_NO_KALLOC); else 0
+int check_loci(const mp_idx_t *mi, int32_t n_seq, int32_t n_loci, const mpb_locus_t *loci);
+// mpb_map_loci on a backend: pairs in batches of up to opt->mini_batch_size residues, each through map_batch over its LocusView with
+// the locus seeding stage; the regions come back in the coordinates of mi's contigs.  Returns check_loci()'s code, or -3 for a backend
+// without locus mode; nothing is mapped then.
+int map_loci(Stages *st, const mp_idx_t *mi, const mp_mapopt_t *opt, int32_t n_seq, const char *const *seqs, const int32_t *lens, const char *const *names,
+             int32_t n_loci, const mpb_locus_t *loci, int32_t *n_reg_out, mp_reg1_t **reg_out);
 
 // ---------------------------------------------------------------- host pipeline (pipeline.cpp, hits.cpp, align.cpp)
 // The --dbg-* switches (mp_dbg_flag, MP_DBG_*) are read once per call.  Their dumps go to stderr, one contiguous block per batch:

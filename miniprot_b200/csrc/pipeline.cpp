@@ -535,4 +535,110 @@ int32_t map_file_multi(Stages *const *st, int n, const mp_idx_t *mi, const char 
 	return 0;
 }
 
+// ---------------------------------------------------------------- locus mode
+
+LocusView::LocusView(const mp_idx_t *mi, int32_t n, const mpb_locus_t *loci) : ctg((size_t)n), bo((size_t)n * 2 + 1)
+{
+	memset(&idx, 0, sizeof(idx));
+	memset(&nt, 0, sizeof(nt));
+	const int32_t bbit = mi->opt.bbit;
+	int64_t acc = 0;
+	for (int32_t q = 0; q < n; ++q) {
+		const mp_ctg_t *c = &mi->nt->ctg[loci[q].cid];
+		mp_ctg_t &v = ctg[(size_t)q];
+		v.off = c->off + loci[q].st, v.len = loci[q].en - loci[q].st, v.name = c->name;
+		const int64_t nb = (v.len + (1 << bbit) - 1) >> bbit; // index.c:11-26
+		bo[(size_t)q * 2] = (uint32_t)acc, acc += nb;
+		bo[(size_t)q * 2 + 1] = (uint32_t)acc, acc += nb;
+	}
+	bo[(size_t)n * 2] = (uint32_t)acc;
+	nt.n_ctg = nt.m_ctg = n, nt.l_seq = nt.m_seq = mi->nt->l_seq, nt.seq = mi->nt->seq, nt.ctg = ctg.data();
+	idx.opt = mi->opt, idx.n_block = (uint32_t)acc, idx.nt = &nt, idx.bo = bo.data();
+}
+
+int check_loci(const mp_idx_t *mi, int32_t n_seq, int32_t n_loci, const mpb_locus_t *loci)
+{
+	if (!mi || !mi->nt || n_seq < 0 || n_loci < 0 || (n_loci > 0 && !loci)) return -1;
+	for (int32_t k = 0; k < n_loci; ++k) {
+		const mpb_locus_t &l = loci[k];
+		if (l.qid < 0 || l.qid >= n_seq || l.cid < 0 || l.cid >= mi->nt->n_ctg || l.st < 0 || l.en > mi->nt->ctg[l.cid].len || l.st >= l.en) return -1;
+	}
+	if (mi->nt->spsc) {
+		fprintf(stderr, "[miniprot_b200] locus mode does not take --spsc splice scores\n");
+		return -3;
+	}
+	if (mp_dbg_flag & ~MP_DBG_NO_KALLOC) {
+		fprintf(stderr, "[miniprot_b200] locus mode does not take the --dbg-* switches (mp_dbg_flag = %#x)\n", (unsigned)mp_dbg_flag);
+		return -3;
+	}
+	return 0;
+}
+
+namespace {
+
+// map_batch's stages in locus mode: S1 is the backend's locus seeding, everything else passes through
+struct LociStages : Stages {
+	Stages *in;
+	explicit LociStages(Stages *s) : in(s) {}
+	void seed_chain(const mp_idx_t *mi, const mp_mapopt_t *opt, const Batch &b, ChainSet &out) override { in->seed_chain_loci(mi, opt, b, out); }
+	void refine(const mp_idx_t *mi, const mp_mapopt_t *opt, const Batch &b, const std::vector<RefineJob> &jobs, RefineSet &out) override { in->refine(mi, opt, b, jobs, out); }
+	void nasw(const mp_idx_t *mi, const ns_opt_t *base, const Batch &b, const std::vector<DpJob> &jobs, DpSet &out) override { in->nasw(mi, base, b, jobs, out); }
+	void batch_begin(const Batch &b) override { in->batch_begin(b); }
+	void batch_end() override { in->batch_end(); }
+	void note_wall(int phase, double ms) override { in->note_wall(phase, ms); }
+	void thread_init() override { in->thread_init(); }
+};
+
+} // namespace
+
+int map_loci(Stages *st, const mp_idx_t *mi, const mp_mapopt_t *opt, int32_t n_seq, const char *const *seqs, const int32_t *lens, const char *const *names,
+             int32_t n_loci, const mpb_locus_t *loci, int32_t *n_reg_out, mp_reg1_t **reg_out)
+{
+	const int rc = check_loci(mi, n_seq, n_loci, loci);
+	if (rc != 0) return rc;
+	for (int32_t k = 0; k < n_loci; ++k) n_reg_out[k] = 0, reg_out[k] = 0;
+	if (n_loci == 0) return 0;
+	LociStages ls(st);
+	for (int32_t i0 = 0; i0 < n_loci;) {
+		// a batch holds pairs until it has mini_batch_size residues (bseq.c:53-74), and fewer than 2^31 blocks
+		int32_t i1 = i0;
+		int64_t residues = 0, blocks = 0;
+		while (i1 < n_loci && residues < opt->mini_batch_size) {
+			const int64_t nb = 2 * ((loci[i1].en - loci[i1].st + (1 << mi->opt.bbit) - 1) >> mi->opt.bbit);
+			if (i1 > i0 && blocks + nb >= (int64_t)1 << 31) break;
+			residues += lens[loci[i1].qid], blocks += nb, ++i1;
+		}
+		const int32_t n = i1 - i0;
+		LocusView v(mi, n, loci + i0);
+		std::vector<const char*> sp((size_t)n), np((size_t)n);
+		std::vector<int32_t> lp((size_t)n);
+		for (int32_t q = 0; q < n; ++q) {
+			const int32_t p = loci[i0 + q].qid;
+			sp[(size_t)q] = seqs[p], lp[(size_t)q] = lens[p], np[(size_t)q] = names ? names[p] : 0;
+		}
+		Batch b;
+		b.n = n, b.seq = sp.data(), b.len = lp.data(), b.name = np.data();
+		if (!st->loci_view(mi, &v.idx)) {
+			fprintf(stderr, "[miniprot_b200] this backend has no locus seeding stage\n");
+			return -3;
+		}
+		map_batch(&ls, &v.idx, opt, b, n_reg_out + i0, reg_out + i0);
+		st->loci_view(0, 0);
+		// locus strand -> contig strand: + adds st, - adds len(cid) - en
+		for (int32_t q = 0; q < n; ++q) {
+			const mpb_locus_t &l = loci[i0 + q];
+			const int64_t clen = mi->nt->ctg[l.cid].len;
+			for (int32_t j = 0; j < n_reg_out[i0 + q]; ++j) {
+				mp_reg1_t *r = &reg_out[i0 + q][j];
+				const uint32_t rev = r->vid & 1;
+				const int64_t sh = rev ? clen - l.en : l.st;
+				r->vid = (uint32_t)l.cid << 1 | rev, r->vs += sh, r->ve += sh;
+				for (int32_t f = 0; f < r->n_feat; ++f) r->feat[f].vs += sh, r->feat[f].ve += sh;
+			}
+		}
+		i0 = i1;
+	}
+	return 0;
+}
+
 } // namespace mpb
