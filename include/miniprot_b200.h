@@ -258,6 +258,33 @@ int mpb_map_loci(mpb_ctx_t *ctx, const mp_idx_t *mi, const mp_mapopt_t *opt, int
                  const int32_t *lens, const char *const *names, int32_t n_loci, const mpb_locus_t *loci,
                  int32_t *n_reg_out, mp_reg1_t **reg_out);
 
+/* An index for locus mode only, from a FASTA or FASTA.gz file (genome, contig table and block offsets as mp_idx_load() sets them,
+ * with the options io, or mp_idxopt_init()'s when io is NULL) or from a .mpi file (its head, as mpb_idx_load_meta(); io is ignored).
+ * Nothing of a k-mer table is built, read or uploaded: ki == kb == NULL, n_kb == 0.  Enough for mpb_map_loci() and
+ * mpb_map_loci_file*(), not for whole-genome mapping.  Free with mp_idx_destroy().  NULL if the file cannot be read. */
+mp_idx_t *mpb_idx_load_genome(const char *fn, const mp_idxopt_t *io);
+
+/* Locus mode over files: proteins from prot_fn (FASTA, gzip allowed, read whole; a repeated name stands for its last record), pairs
+ * from loci_fn, a TSV of `protein contig start end` (0-based, end exclusive; blank lines and lines starting with '#' skipped).  For
+ * every pair, in file order, writes what the reference CLI prints with the same options when that locus alone is the genome --
+ * PAF with or without cs, --gff / --gff-only / --gtf, --aln, --trans, -P, --gff-delim, --max-intron-out, -u, --outn / --outs /
+ * --outc applied per pair -- moved to the real contig: its name and length in PAF columns 6-7 (and in the ##PAF lines), start and
+ * end moved by st in PAF columns 8-9 and GFF / GTF columns 4-5, the contig's name in GFF / GTF column 1.  The output as a whole is
+ * one file: "##gff-version 3" once at the top with --gff, and one counter numbers the ids of all pairs.  Genome bases past a locus
+ * end are never read (--aln's codon after a hit is clipped there, as in the reference given the locus alone).
+ * Everything is validated before anything is written.  Returns 0; -1 (with "file:line: why" on stderr) for an unreadable file, a
+ * malformed line, an unknown protein or contig or a range outside 0 <= start < end <= contig length, and for a null, missing or
+ * repeated context; -3 (with a message) for what mpb_map_loci() refuses; -2 when out_path cannot be created.
+ * _multi: over n_ctx distinct contexts as mpb_map_file_multi() (units of at most mini_batch_size / n_ctx residues, one mapper thread
+ * per context, written in input order); the output is the same byte for byte for any n_ctx and mini_batch_size.  The genome is made
+ * resident in every context (the packed genome and the contig table only, unless the context holds the whole index). */
+int32_t mpb_map_loci_file(mpb_ctx_t *ctx, const mp_idx_t *mi, const char *prot_fn, const char *loci_fn, const mp_mapopt_t *opt, FILE *out);
+int32_t mpb_map_loci_file_path(mpb_ctx_t *ctx, const mp_idx_t *mi, const char *prot_fn, const char *loci_fn, const mp_mapopt_t *opt, const char *out_path);
+int32_t mpb_map_loci_file_multi(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_idx_t *mi, const char *prot_fn, const char *loci_fn, const mp_mapopt_t *opt,
+                                FILE *out);
+int32_t mpb_map_loci_file_multi_path(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_idx_t *mi, const char *prot_fn, const char *loci_fn,
+                                     const mp_mapopt_t *opt, const char *out_path);
+
 /* mp_map_file() with an explicit output stream and context (tests, benchmarks). */
 int32_t mpb_map_file(mpb_ctx_t *ctx, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, FILE *out);
 /* mpb_map_file() over n_ctx distinct contexts (on one or several GPUs) at once: the input is cut into units of at most

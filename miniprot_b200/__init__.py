@@ -215,6 +215,12 @@ def lib() -> C.CDLL:
         L.mpb_map_file_path.argtypes = [C.c_void_p, C.POINTER(Idx), C.c_char_p, C.POINTER(MapOpt), C.c_char_p]
         L.mpb_map_file_multi_path.restype = C.c_int32
         L.mpb_map_file_multi_path.argtypes = [C.POINTER(C.c_void_p), C.c_int32, C.POINTER(Idx), C.c_char_p, C.POINTER(MapOpt), C.c_char_p]
+        L.mpb_idx_load_genome.restype = C.POINTER(Idx)
+        L.mpb_idx_load_genome.argtypes = [C.c_char_p, C.POINTER(IdxOpt)]
+        L.mpb_map_loci_file_multi.restype = C.c_int32
+        L.mpb_map_loci_file_multi.argtypes = [C.POINTER(C.c_void_p), C.c_int32, C.POINTER(Idx), C.c_char_p, C.c_char_p, C.POINTER(MapOpt), C.c_void_p]
+        L.mpb_map_loci_file_multi_path.restype = C.c_int32
+        L.mpb_map_loci_file_multi_path.argtypes = [C.POINTER(C.c_void_p), C.c_int32, C.POINTER(Idx), C.c_char_p, C.c_char_p, C.POINTER(MapOpt), C.c_char_p]
         L.mpb_idx_share.argtypes = [C.c_void_p, C.c_void_p]
         L.mpb_event_begin.argtypes = [C.c_void_p]
         L.mpb_event_end_ms.restype = C.c_double
@@ -327,6 +333,38 @@ def map_file_multi(ctxs, mi, prot_path: str, out_path: str, mo: MapOpt | None = 
     rc = lib().mpb_map_file_multi_path(arr, len(ctxs), mi, prot_path.encode(), C.byref(mo), out_path.encode())
     if rc != 0:
         raise RuntimeError(f"mpb_map_file_multi failed ({rc})")
+
+
+def idx_load_genome(path: str, io: IdxOpt | None = None):
+    """mpb_idx_load_genome: an index for locus mode only (genome and contig table of a FASTA, or the head of a .mpi file; no k-mer
+    table)."""
+    mi = lib().mpb_idx_load_genome(path.encode(), C.byref(io) if io is not None else None)
+    if not mi:
+        raise RuntimeError(f"cannot read a genome from {path}")
+    return mi
+
+
+def map_loci_file(ctxs, mi, prot_path: str, loci_path: str, out_path: str = "-", mo: MapOpt | None = None) -> None:
+    """mpb_map_loci_file_multi: proteins (FASTA) against the loci of a TSV (`protein contig start end`) on one Context or a list of
+    distinct ones, in the output format of `mo`; out_path "-" is this process's standard output."""
+    mo = mo or mapopt()
+    ctxs = [ctxs] if isinstance(ctxs, Context) else list(ctxs)
+    arr = (C.c_void_p * len(ctxs))(*[c.h for c in ctxs])
+    L = lib()
+    if out_path == "-":
+        import sys
+
+        sys.stdout.flush()
+        libc = C.CDLL(None)
+        libc.fdopen.restype, libc.fdopen.argtypes = C.c_void_p, [C.c_int, C.c_char_p]
+        libc.fclose.argtypes = [C.c_void_p]
+        fp = libc.fdopen(os.dup(sys.stdout.fileno()), b"wb")
+        rc = L.mpb_map_loci_file_multi(arr, len(ctxs), mi, prot_path.encode(), loci_path.encode(), C.byref(mo), fp)
+        libc.fclose(fp)
+    else:
+        rc = L.mpb_map_loci_file_multi_path(arr, len(ctxs), mi, prot_path.encode(), loci_path.encode(), C.byref(mo), out_path.encode())
+    if rc != 0:
+        raise RuntimeError(f"mpb_map_loci_file failed ({rc})")
 
 
 def nsopt(mat=None, **over) -> NsOpt:

@@ -97,15 +97,16 @@ void format_gtf(Str &o, const mp_idx_t *mi, const mp_mapopt_t *opt, const char *
 }
 
 // --aln / --trans (format.c:189-331): four aligned text rows (genome bases, their translation, match line, protein residues:
-// "##ATN", "##ATA", "##AAS", "##AQA") and the translated protein ("##STA"); long introns are abbreviated to their flanks
-void format_residue(Str &o, const mp_idx_t *mi, const mp_mapopt_t *opt, const char *qseq, const mp_reg1_t *r)
+// "##ATN", "##ATA", "##AAS", "##AQA") and the translated protein ("##STA"); long introns are abbreviated to their flanks.
+// The one read of the genome past the hit: the codon after r->ve (format.c:219), clipped at the contig end or at nt_lim (>= 0).
+void format_residue(Str &o, const mp_idx_t *mi, const mp_mapopt_t *opt, const char *qseq, const mp_reg1_t *r, int64_t nt_lim)
 {
 	static const char UC[] = "ACGTN", LC[] = "acgtn";
 	const mp_extra_t *e = r->p;
 	if (!e) return;
 	const int32_t max_flank = opt->max_intron_flank;
 	std::vector<uint8_t> nt((size_t)(r->ve - r->vs + 3));
-	const int64_t l_nt = nt_fetch_v(mi->nt, r->vid, r->vs, r->ve + 3, nt.data());
+	const int64_t l_nt = nt_fetch_v(mi->nt, r->vid, r->vs, nt_lim >= 0 && nt_lim < r->ve + 3 ? nt_lim : r->ve + 3, nt.data());
 	std::string atn = "##ATN\t", ata = "##ATA\t", aas = "##AAS\t", aqa = "##AQA\t", sta = "##STA\t";
 	auto col = [&](char a, char b, char c, char d) { atn += a, ata += b, aas += c, aqa += d; };
 	auto codon_cols = [&](int32_t i, char match, char res, bool translate) { // three columns of one genome codon
@@ -177,16 +178,16 @@ void format_residue(Str &o, const mp_idx_t *mi, const mp_mapopt_t *opt, const ch
 
 // everything the reference prints for one hit, in its order (format.c:453-473); r == 0: the unmapped line of -u
 void format_output(Str &o, const mp_idx_t *mi, const mp_mapopt_t *opt, const char *qname, int32_t qlen, const char *qseq, const mp_reg1_t *r, int64_t id,
-                   int32_t hit_idx)
+                   int32_t hit_idx, int64_t nt_lim)
 {
 	if (!r) {
 		if (opt->flag & MP_F_SHOW_UNMAP) format_hit(o, mi, opt, qname, qlen, qseq, 0);
 	} else if (opt->flag & MP_F_GTF) {
-		if (opt->flag & (MP_F_SHOW_RESIDUE | MP_F_SHOW_TRANS)) format_hit(o, mi, opt, qname, qlen, qseq, r), format_residue(o, mi, opt, qseq, r);
+		if (opt->flag & (MP_F_SHOW_RESIDUE | MP_F_SHOW_TRANS)) format_hit(o, mi, opt, qname, qlen, qseq, r), format_residue(o, mi, opt, qseq, r, nt_lim);
 		format_gtf(o, mi, opt, qname, qlen, r, id);
 	} else {
 		if (!(opt->flag & MP_F_NO_PAF)) format_hit(o, mi, opt, qname, qlen, qseq, r);
-		if (opt->flag & (MP_F_SHOW_RESIDUE | MP_F_SHOW_TRANS)) format_residue(o, mi, opt, qseq, r);
+		if (opt->flag & (MP_F_SHOW_RESIDUE | MP_F_SHOW_TRANS)) format_residue(o, mi, opt, qseq, r, nt_lim);
 		if (opt->flag & MP_F_GFF) format_gff(o, mi, opt, qname, qlen, r, id, hit_idx);
 	}
 }

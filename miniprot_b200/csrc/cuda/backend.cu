@@ -782,6 +782,61 @@ int32_t mpb_map_file_multi_path(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_i
 	return rc;
 }
 
+// the locus file driver on n_ctx contexts, into `out` or, when that is null, into a file created at out_path once the input is valid
+static int32_t map_loci_file_on(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_idx_t *mi, const char *prot_fn, const char *loci_fn, const mp_mapopt_t *opt,
+                                FILE *out, const char *out_path)
+{
+	if (!ctx || n_ctx < 1 || !opt || !mi) return -1;
+	std::vector<mpb_ctx_s*> by_addr(ctx, ctx + n_ctx);
+	std::sort(by_addr.begin(), by_addr.end());
+	if (by_addr[0] == 0 || std::adjacent_find(by_addr.begin(), by_addr.end()) != by_addr.end()) return -1; // a context maps one unit at a time
+	LociFile in;
+	int32_t rc = loci_file_read(mi, prot_fn, loci_fn, in);
+	if (rc != 0) return rc;
+	if (bad_scoring(opt->go, opt->ie_coef) || bad_index(mi)) return -3;
+	FILE *fp = out ? out : fopen(out_path, "wb");
+	if (!fp) return -2;
+	{
+		std::vector<std::unique_lock<std::mutex>> held;
+		for (mpb_ctx_s *c : by_addr) held.emplace_back(c->mu); // in address order, as mpb_map_file_multi
+		// the genome is resident in every context before the mappers start (the whole index where a context holds it already)
+		for (int32_t k = 0; k < n_ctx && rc == 0; ++k)
+			if (acquire_genome(ctx[k], mi) != 0) {
+				fprintf(stderr, "[miniprot_b200] the index has no genome on the host and is not resident in the context\n");
+				rc = -1;
+			}
+		std::vector<Stages*> st((size_t)n_ctx);
+		for (int32_t k = 0; k < n_ctx; ++k) st[(size_t)k] = ctx[k]->stages;
+		if (rc == 0) {
+			MPB_CUDA_OK(cudaSetDevice(ctx[0]->device));
+			rc = map_loci_file(st.data(), n_ctx, mi, in, opt, fp);
+		}
+	}
+	if (!out) fclose(fp);
+	return rc;
+}
+
+int32_t mpb_map_loci_file(mpb_ctx_t *c, const mp_idx_t *mi, const char *prot_fn, const char *loci_fn, const mp_mapopt_t *opt, FILE *out)
+{
+	return out ? map_loci_file_on(&c, 1, mi, prot_fn, loci_fn, opt, out, 0) : -1;
+}
+
+int32_t mpb_map_loci_file_path(mpb_ctx_t *c, const mp_idx_t *mi, const char *prot_fn, const char *loci_fn, const mp_mapopt_t *opt, const char *out_path)
+{
+	return out_path ? map_loci_file_on(&c, 1, mi, prot_fn, loci_fn, opt, 0, out_path) : -1;
+}
+
+int32_t mpb_map_loci_file_multi(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_idx_t *mi, const char *prot_fn, const char *loci_fn, const mp_mapopt_t *opt, FILE *out)
+{
+	return out ? map_loci_file_on(ctx, n_ctx, mi, prot_fn, loci_fn, opt, out, 0) : -1;
+}
+
+int32_t mpb_map_loci_file_multi_path(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_idx_t *mi, const char *prot_fn, const char *loci_fn, const mp_mapopt_t *opt,
+                                     const char *out_path)
+{
+	return out_path ? map_loci_file_on(ctx, n_ctx, mi, prot_fn, loci_fn, opt, 0, out_path) : -1;
+}
+
 mp_reg1_t *mp_map(const mp_idx_t *mi, int qlen, const char *seq, int *n_reg, mp_tbuf_t *, const mp_mapopt_t *opt, const char *qname)
 {
 	mp_reg1_t *reg = 0;

@@ -234,6 +234,33 @@ mp_idx_t *mp_idx_load(const char *fn, const mp_idxopt_t *io, int32_t n_threads) 
 	return idx_build(fn, io, n_threads);
 }
 
+// An index for locus mode only: the genome, contig table and block offsets of a FASTA (io's options, mp_idxopt_init's without io), or
+// the head of a .mpi file (options as stored, io ignored).  No k-mer table is built or read: ki == kb == NULL, n_kb == 0.
+mp_idx_t *mpb_idx_load_genome(const char *fn, const mp_idxopt_t *io)
+{
+	if (!fn) return 0;
+	FILE *fp = fopen(fn, "rb");
+	if (!fp) return 0;
+	char magic[4];
+	const size_t got = fread(magic, 1, 4, fp);
+	if (got == 4 && memcmp(magic, MP_IDX_MAGIC, 3) == 0 && magic[3] <= MP_IDX_MAGIC[3]) {
+		rewind(fp);
+		mp_idx_t *mi = idx_restore_head(fp);
+		fclose(fp);
+		if (mi) mi->n_kb = 0;
+		return mi;
+	}
+	fclose(fp);
+	mp_ntdb_t *nt = ntdb_read_fasta(fn);
+	if (!nt) return 0;
+	mp_idx_t *mi = (mp_idx_t*)calloc(1, sizeof(mp_idx_t));
+	if (io) mi->opt = *io;
+	else mp_idxopt_init(&mi->opt);
+	mi->nt = nt;
+	mi->bo = block_offsets(nt, mi->opt.bbit, &mi->n_block);
+	return mi;
+}
+
 void mp_idx_print_stat(const mp_idx_t *mi, int32_t max_occ) // index.c:138-152
 {
 	const uint32_t n = idx_n_bucket(&mi->opt);

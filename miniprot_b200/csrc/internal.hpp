@@ -5,6 +5,7 @@
 #include <stdlib.h>
 #include <string.h>
 #include <string>
+#include <unordered_map>
 #include <vector>
 #include "miniprot_b200.h"
 #include "flagsort.hpp"
@@ -140,6 +141,24 @@ int check_loci(const mp_idx_t *mi, int32_t n_seq, int32_t n_loci, const mpb_locu
 // without locus mode; nothing is mapped then.
 int map_loci(Stages *st, const mp_idx_t *mi, const mp_mapopt_t *opt, int32_t n_seq, const char *const *seqs, const int32_t *lens, const char *const *names,
              int32_t n_loci, const mpb_locus_t *loci, int32_t *n_reg_out, mp_reg1_t **reg_out);
+// The inputs of the locus file driver, read whole: proteins (a repeated name stands for its last record) and the pairs of the loci
+// file in its order.
+struct LociFile {
+	std::vector<std::string> names, seqs;
+	std::vector<const char*> sp, np;
+	std::vector<int32_t> len;
+	std::vector<mpb_locus_t> loci;
+	std::unordered_map<std::string, int32_t> qid;
+	void add_protein(const std::string &name, const std::string &seq);
+};
+// Reads prot_fn (FASTA, gzip or plain) and loci_fn (`protein contig start end` per line, 0-based, end exclusive; blank and '#' lines
+// skipped).  -1 with "file:line: why" on stderr for an unreadable file, a malformed line, an unknown protein or contig, or a bad
+// range; then check_loci()'s -3 refusals; else 0.
+int loci_file_read(const mp_idx_t *mi, const char *prot_fn, const char *loci_fn, LociFile &in);
+// mpb_map_loci_file_multi on n backends: for every pair, in file order, the output of the reference given that locus alone as the
+// genome, in contig coordinates; ids numbered over the whole output.  Returns 0, or -3 (nothing written) for a backend without
+// locus mode.
+int32_t map_loci_file(Stages *const *st, int n, const mp_idx_t *mi, const LociFile &in, const mp_mapopt_t *opt, FILE *out);
 
 // ---------------------------------------------------------------- host pipeline (pipeline.cpp, hits.cpp, align.cpp)
 // The --dbg-* switches (mp_dbg_flag, MP_DBG_*) are read once per call.  Their dumps go to stderr, one contiguous block per batch:
@@ -164,9 +183,10 @@ struct Str {                      // growable output buffer
 void format_hit(Str &out, const mp_idx_t *mi, const mp_mapopt_t *opt, const char *qname, int32_t qlen, const char *qseq,
                 const mp_reg1_t *r);
 // everything the reference prints for one hit (PAF, --aln / --trans blocks, GFF3 or GTF, format.c:453); id = running number of
-// the hit in the whole output, hit_idx = its rank for this protein (1-based); r == 0: the unmapped line of -u
+// the hit in the whole output, hit_idx = its rank for this protein (1-based); r == 0: the unmapped line of -u.  nt_lim >= 0: the
+// genome on strand r->vid ends there for this hit (the end of its locus in locus mode); the only read past r->ve is --aln's codon.
 void format_output(Str &out, const mp_idx_t *mi, const mp_mapopt_t *opt, const char *qname, int32_t qlen, const char *qseq,
-                   const mp_reg1_t *r, int64_t id, int32_t hit_idx);
+                   const mp_reg1_t *r, int64_t id, int32_t hit_idx, int64_t nt_lim = -1);
 
 // hits.cpp (hit.c)
 mp_reg1_t *regs_from_chains(const mp_idx_t *mi, int32_t n_u, const uint64_t *u, const uint64_t *a, int32_t *n_reg); // hit.c:32

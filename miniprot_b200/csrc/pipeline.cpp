@@ -18,6 +18,7 @@
 #include <chrono>
 #include <condition_variable>
 #include <deque>
+#include <errno.h>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -278,8 +279,10 @@ void map_batch(Stages *st, const mp_idx_t *mi, const mp_mapopt_t *opt, const Bat
 // map.c:293-326: per protein, hits in rank order subject to --outn / --outs / --outc; unmapped line with -u.  Every printed hit
 // gets the next number of a counter that runs over the whole file (the MP%06d ids of GFF / GTF, map.c:306): the hits each
 // protein will print are counted first, so that formatting -- independent per protein -- can run on the worker pool, each range
-// into its own buffer, written in order.
-static void write_batch(FILE *out, const mp_idx_t *mi, const mp_mapopt_t *opt, const Batch &b, const int32_t *n_reg, mp_reg1_t *const *reg, int64_t *id_counter)
+// into its own buffer, written in order.  loci (locus mode): query q is the protein of locus loci[q], whose hits are in contig
+// coordinates but must not read the genome past the locus end (format_output's nt_lim), as the reference given the locus alone.
+static void write_batch(FILE *out, const mp_idx_t *mi, const mp_mapopt_t *opt, const Batch &b, const int32_t *n_reg, mp_reg1_t *const *reg, int64_t *id_counter,
+                        const mpb_locus_t *loci = 0)
 {
 	auto printed = [&](int32_t q, int32_t j, int32_t best) {
 		const mp_reg1_t *r = &reg[q][j];
@@ -305,7 +308,9 @@ static void write_batch(FILE *out, const mp_idx_t *mi, const mp_mapopt_t *opt, c
 			for (int32_t j = 0; j < n_reg[q] && j < opt->out_n; ++j) {
 				if (!printed(q, j, best)) continue;
 				++n_out;
-				format_output(buf, mi, opt, b.name[q], b.len[q], b.seq[q], &reg[q][j], id0[(size_t)q] + n_out, j + 1);
+				int64_t nt_lim = -1; // locus end on the hit's strand: en on +, len(cid) - st on -
+				if (loci) nt_lim = (reg[q][j].vid & 1) ? mi->nt->ctg[loci[q].cid].len - loci[q].st : loci[q].en;
+				format_output(buf, mi, opt, b.name[q], b.len[q], b.seq[q], &reg[q][j], id0[(size_t)q] + n_out, j + 1, nt_lim);
 			}
 			if (n_out == 0) format_output(buf, mi, opt, b.name[q], b.len[q], b.seq[q], 0, 0, 0);
 		}
@@ -314,6 +319,16 @@ static void write_batch(FILE *out, const mp_idx_t *mi, const mp_mapopt_t *opt, c
 		if (part[(size_t)c].l) fwrite(part[(size_t)c].s, 1, (size_t)part[(size_t)c].l, out);
 		free(part[(size_t)c].s);
 	}
+}
+
+// hits are libc-allocated like the reference's (map.c:314-318)
+static void release_regs(const std::vector<int32_t> &n_reg, std::vector<mp_reg1_t*> &reg)
+{
+	for (size_t i = 0; i < reg.size(); ++i) {
+		for (int32_t j = 0; j < n_reg[i]; ++j) free(reg[i][j].feat), free(reg[i][j].p);
+		free(reg[i]);
+	}
+	reg.clear();
 }
 
 // One mini-batch of the query file with everything that must live from the reader to the writer.
@@ -328,14 +343,7 @@ struct FileBatch {
 		b.n = (int32_t)seqs.size(), b.seq = sp.data(), b.len = len.data(), b.name = np.data();
 		return b;
 	}
-	void release() // hits are libc-allocated like the reference's (map.c:314-318)
-	{
-		for (size_t i = 0; i < reg.size(); ++i) {
-			for (int32_t j = 0; j < n_reg[i]; ++j) free(reg[i][j].feat), free(reg[i][j].p);
-			free(reg[i]);
-		}
-		reg.clear();
-	}
+	void release() { release_regs(n_reg, reg); }
 };
 
 // bseq.c:53-74: records until the batch holds mini_batch_size residues; null at the end of the input
@@ -639,6 +647,182 @@ int map_loci(Stages *st, const mp_idx_t *mi, const mp_mapopt_t *opt, int32_t n_s
 		i0 = i1;
 	}
 	return 0;
+}
+
+// ---------------------------------------------------------------- locus mode: the file driver
+
+void LociFile::add_protein(const std::string &name, const std::string &seq)
+{
+	auto it = qid.find(name);
+	if (it != qid.end()) { // the last record of a name is the one its loci are aligned to
+		seqs[(size_t)it->second] = seq;
+		return;
+	}
+	qid.emplace(name, (int32_t)names.size());
+	names.push_back(name), seqs.push_back(seq);
+}
+
+int loci_file_read(const mp_idx_t *mi, const char *prot_fn, const char *loci_fn, LociFile &in)
+{
+	if (!mi || !mi->nt || !prot_fn || !loci_fn) return -1;
+	{
+		FastxReader rd(prot_fn);
+		if (!rd.fp) {
+			fprintf(stderr, "[miniprot_b200] %s: cannot open the protein file\n", prot_fn);
+			return -1;
+		}
+		std::string name, seq;
+		while (rd.next(name, seq)) in.add_protein(name, seq);
+	}
+	in.sp.resize(in.seqs.size()), in.np.resize(in.seqs.size()), in.len.resize(in.seqs.size());
+	for (size_t i = 0; i < in.seqs.size(); ++i) in.sp[i] = in.seqs[i].c_str(), in.np[i] = in.names[i].c_str(), in.len[i] = (int32_t)in.seqs[i].size();
+	std::unordered_map<std::string, int32_t> cid;
+	for (int32_t i = 0; i < mi->nt->n_ctg; ++i) cid[mi->nt->ctg[i].name] = i;
+	FILE *fp = fopen(loci_fn, "r");
+	if (!fp) {
+		fprintf(stderr, "[miniprot_b200] %s: cannot open the loci file\n", loci_fn);
+		return -1;
+	}
+	char *line = 0;
+	size_t cap = 0;
+	int rc = 0;
+	for (long ln = 1; getline(&line, &cap, fp) >= 0; ++ln) {
+		std::vector<char*> t; // whitespace-separated fields
+		for (char *q = line; *q;) {
+			while (*q && isspace((unsigned char)*q)) ++q;
+			if (!*q) break;
+			t.push_back(q);
+			while (*q && !isspace((unsigned char)*q)) ++q;
+			if (*q) *q++ = 0;
+		}
+		if (t.empty() || t[0][0] == '#') continue;
+		int64_t v[2] = { 0, 0 };
+		bool num = t.size() >= 4;
+		for (int k = 0; k < 2 && num; ++k) {
+			char *end;
+			errno = 0;
+			v[k] = strtoll(t[2 + (size_t)k], &end, 10);
+			num = *end == 0 && errno == 0;
+		}
+		const char *why = 0;
+		if (!num) why = "expected `protein contig start end` with integer start and end";
+		else if (!in.qid.count(t[0])) why = "unknown protein";
+		else if (!cid.count(t[1])) why = "unknown contig";
+		else if (v[0] < 0 || v[0] >= v[1] || v[1] > mi->nt->ctg[cid[t[1]]].len) why = "the range is not 0 <= start < end <= contig length";
+		if (why) {
+			fprintf(stderr, "[miniprot_b200] %s:%ld: %s\n", loci_fn, ln, why);
+			rc = -1;
+			break;
+		}
+		mpb_locus_t l;
+		l.qid = in.qid[t[0]], l.cid = cid[t[1]], l.st = v[0], l.en = v[1];
+		in.loci.push_back(l);
+	}
+	free(line);
+	fclose(fp);
+	if (rc != 0) return rc;
+	return check_loci(mi, (int32_t)in.seqs.size(), (int32_t)in.loci.size(), in.loci.data());
+}
+
+namespace {
+
+// pairs [i0, i0 + n) of a loci file and their hits, from the mapper that aligned them to the writer
+struct LociUnit {
+	int32_t i0 = 0, n = 0;
+	std::vector<int32_t> n_reg;
+	std::vector<mp_reg1_t*> reg;
+	int rc = 0;
+	void release() { release_regs(n_reg, reg); }
+};
+
+} // namespace
+
+// map_file_multi's pipeline over the pairs of a loci file, which are in memory already: the pairs are cut into units of at most
+// mini_batch_size / n residues (at least one pair), n mapper threads -- one per backend -- take the next unit each and align it
+// with map_loci, and the calling thread writes the units in input order and owns the hit counter.  At most 2n units are between
+// the mappers and the writer.  With one backend, a single unit or MPB_FILE_PIPELINE=0 (one backend) runs everything on the
+// calling thread.  Hits do not depend on unit boundaries (map_loci), so neither does the output.
+int32_t map_loci_file(Stages *const *st, int n, const mp_idx_t *mi, const LociFile &in, const mp_mapopt_t *opt, FILE *out)
+{
+	if (n < 1) return -1;
+	for (int k = 0; k < n; ++k)
+		if (!st[k]->loci_view(0, 0)) {
+			fprintf(stderr, "[miniprot_b200] this backend has no locus seeding stage\n");
+			return -3;
+		}
+	const int32_t n_loci = (int32_t)in.loci.size();
+	const int64_t unit_size = std::max<int64_t>(1, opt->mini_batch_size / n);
+	std::vector<std::unique_ptr<LociUnit>> units;
+	for (int32_t i0 = 0; i0 < n_loci;) {
+		int32_t i1 = i0;
+		for (int64_t residues = 0; i1 < n_loci && residues < unit_size; ++i1) residues += in.len[(size_t)in.loci[(size_t)i1].qid];
+		units.emplace_back(new LociUnit);
+		units.back()->i0 = i0, units.back()->n = i1 - i0;
+		i0 = i1;
+	}
+	if (opt->flag & MP_F_GFF) fputs("##gff-version 3\n", out); // map.c:338
+	auto map_step = [&](Stages *s, LociUnit &u) {
+		u.n_reg.assign((size_t)u.n, 0), u.reg.assign((size_t)u.n, (mp_reg1_t*)0);
+		u.rc = map_loci(s, mi, opt, (int32_t)in.seqs.size(), in.sp.data(), in.len.data(), in.np.data(), u.n, in.loci.data() + u.i0, u.n_reg.data(), u.reg.data());
+	};
+	int64_t id_counter = 0;
+	int32_t rc = 0;
+	auto write_step = [&](LociUnit &u) {
+		if (u.rc != 0 && rc == 0) rc = u.rc;
+		std::vector<const char*> sp((size_t)u.n), np((size_t)u.n);
+		std::vector<int32_t> lp((size_t)u.n);
+		for (int32_t k = 0; k < u.n; ++k) {
+			const int32_t q = in.loci[(size_t)(u.i0 + k)].qid;
+			sp[(size_t)k] = in.sp[(size_t)q], np[(size_t)k] = in.np[(size_t)q], lp[(size_t)k] = in.len[(size_t)q];
+		}
+		Batch b;
+		b.n = u.n, b.seq = sp.data(), b.len = lp.data(), b.name = np.data();
+		write_batch(out, mi, opt, b, u.n_reg.data(), u.reg.data(), &id_counter, in.loci.data() + u.i0);
+		u.release();
+	};
+	const char *e = getenv("MPB_FILE_PIPELINE");
+	if (n == 1 && ((e && atoi(e) == 0) || units.size() <= 1)) {
+		for (std::unique_ptr<LociUnit> &u : units) map_step(st[0], *u), write_step(*u), u.reset();
+		return rc;
+	}
+	const size_t max_in_flight = 2 * (size_t)n;
+	std::mutex mu;
+	std::condition_variable cv;
+	size_t n_taken = 0, n_written = 0;
+	std::vector<char> mapped(units.size(), 0);
+	std::vector<std::thread> mappers;
+	for (int k = 0; k < n; ++k)
+		mappers.emplace_back([&, k] {
+			st[k]->thread_init();
+			for (;;) {
+				size_t u;
+				{
+					std::unique_lock<std::mutex> lk(mu);
+					cv.wait(lk, [&] { return n_taken == units.size() || n_taken - n_written < max_in_flight; });
+					if (n_taken == units.size()) return;
+					u = n_taken++;
+				}
+				map_step(st[k], *units[u]);
+				if (mp_verbose >= 3)
+					fprintf(stderr, "[M::%s::%.3f*%.2f] aligned %d pairs (context %d)\n", "map_loci_file", mp_realtime(), mp_cputime() / mp_realtime(), units[u]->n, k);
+				std::lock_guard<std::mutex> lk(mu);
+				mapped[u] = 1;
+				cv.notify_all();
+			}
+		});
+	for (size_t w = 0; w < units.size(); ++w) {
+		{
+			std::unique_lock<std::mutex> lk(mu);
+			cv.wait(lk, [&] { return mapped[w] != 0; });
+		}
+		write_step(*units[w]);
+		units[w].reset();
+		std::lock_guard<std::mutex> lk(mu);
+		++n_written;
+		cv.notify_all();
+	}
+	for (std::thread &t : mappers) t.join();
+	return rc;
 }
 
 } // namespace mpb
