@@ -285,12 +285,15 @@ int32_t mpb_map_loci_file_multi(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_i
 int32_t mpb_map_loci_file_multi_path(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_idx_t *mi, const char *prot_fn, const char *loci_fn,
                                      const mp_mapopt_t *opt, const char *out_path);
 
-/* mp_map_file() with an explicit output stream and context (tests, benchmarks). */
+/* mp_map_file() with an explicit output stream and context (tests, benchmarks).  The index is made resident in the context before
+ * anything is mapped: shared from another context that holds it, else uploaded from its host tables.  Returns 0; -1 for a null
+ * context, an unreadable input, or an index that has no host tables (mpb_idx_load_device) and is held by no context (with a
+ * message); -3 (with a message) for refused options.  mpb_map_file_multi(&ctx, 1, ...). */
 int32_t mpb_map_file(mpb_ctx_t *ctx, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, FILE *out);
 /* mpb_map_file() over n_ctx distinct contexts (on one or several GPUs) at once: the input is cut into units of at most
  * mini_batch_size / n_ctx residues, each context maps the next unit on a thread of its own, and the output is written in input
  * order -- byte for byte what mpb_map_file() writes.  The index is made resident in every context first (shared from one that holds
- * it, else uploaded).  Returns what mpb_map_file() returns; -1 also for a repeated or null context.  n_ctx == 1 is mpb_map_file(). */
+ * it, else uploaded).  Returns what mpb_map_file() returns; -1 also for a repeated or null context. */
 int32_t mpb_map_file_multi(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, FILE *out);
 int32_t mpb_map_file_multi_path(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, const char *out_path);
 /* Format one hit exactly like the reference's PAF writer (format.c:333); appends to a malloc'ed buffer. */

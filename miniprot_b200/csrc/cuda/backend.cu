@@ -488,6 +488,39 @@ struct AnyCtx {
 	~AnyCtx() { if (pool) pool->release(c); }
 };
 
+// The contexts of one call of a file entry point
+struct FileCtx {
+	std::vector<mpb_ctx_s*> ctx, by_addr;
+	std::vector<std::unique_lock<std::mutex>> held;
+	std::vector<Stages*> st; // after hold(): the contexts' stages, in the caller's order
+	// false unless the n contexts are non-null and distinct: a context maps one unit at a time
+	bool distinct(mpb_ctx_t *const *c, int32_t n)
+	{
+		if (!c || n < 1) return false;
+		ctx.assign(c, c + n), by_addr = ctx;
+		std::sort(by_addr.begin(), by_addr.end());
+		return by_addr[0] && std::adjacent_find(by_addr.begin(), by_addr.end()) == by_addr.end();
+	}
+	// After distinct(): holds the contexts' mutexes in address order until destruction (two such calls never wait for each other in a
+	// cycle), makes mi resident in every context before the mappers start -- the whole index (shared between contexts where one holds
+	// it), or only its genome when genome_only (locus mode) -- and makes the first context's device current.  -1 with a message when
+	// mi cannot be made resident.
+	int hold(const mp_idx_t *mi, bool genome_only)
+	{
+		for (mpb_ctx_s *c : by_addr) held.emplace_back(c->mu);
+		for (mpb_ctx_s *c : ctx) {
+			if (genome_only ? acquire_genome(c, mi) != 0 : acquire_index(c, mi) != 0) {
+				fprintf(stderr, genome_only ? "[miniprot_b200] the index has no genome on the host and is not resident in the context\n"
+				                            : "[miniprot_b200] the index is neither resident in a context nor on the host\n");
+				return -1;
+			}
+			st.push_back(c->stages);
+		}
+		MPB_CUDA_OK(cudaSetDevice(ctx[0]->device));
+		return 0;
+	}
+};
+
 } // namespace
 
 extern "C" {
@@ -736,41 +769,21 @@ int mpb_seed_loci_batch(mpb_ctx_t *c, const mp_idx_t *mi, int32_t max_occ, int32
 
 int32_t mpb_map_file(mpb_ctx_t *c, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, FILE *out)
 {
-	if (!c) return -1;
-	if (bad_scoring(opt->go, opt->ie_coef) || bad_index(mi) || bad_dbg_flags(opt)) return -3;
-	std::lock_guard<std::mutex> cl(c->mu);
-	MPB_CUDA_OK(cudaSetDevice(c->device));
-	return map_file(c->stages, mi, fn, opt, out);
+	return mpb_map_file_multi(&c, 1, mi, fn, opt, out);
 }
 
 int32_t mpb_map_file_path(mpb_ctx_t *c, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, const char *out_path)
 {
-	FILE *fp = fopen(out_path, "wb");
-	if (!fp) return -2;
-	int32_t rc = mpb_map_file(c, mi, fn, opt, fp);
-	fclose(fp);
-	return rc;
+	return mpb_map_file_multi_path(&c, 1, mi, fn, opt, out_path);
 }
 
 int32_t mpb_map_file_multi(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, FILE *out)
 {
-	if (!ctx || n_ctx < 1) return -1;
-	std::vector<mpb_ctx_s*> by_addr(ctx, ctx + n_ctx);
-	std::sort(by_addr.begin(), by_addr.end());
-	if (by_addr[0] == 0 || std::adjacent_find(by_addr.begin(), by_addr.end()) != by_addr.end()) return -1; // a context maps one unit at a time
-	if (n_ctx == 1) return mpb_map_file(ctx[0], mi, fn, opt, out);
+	FileCtx fc;
+	if (!fc.distinct(ctx, n_ctx)) return -1;
 	if (bad_scoring(opt->go, opt->ie_coef) || bad_index(mi) || bad_dbg_flags(opt)) return -3;
-	std::vector<std::unique_lock<std::mutex>> held;
-	for (mpb_ctx_s *c : by_addr) held.emplace_back(c->mu); // in address order: two such calls never wait for each other in a cycle
-	// the index is resident in every context before the mappers start: in the first one that holds it or can upload it, shared
-	// from there to the others (on the same device nothing is copied)
-	for (int32_t k = 0; k < n_ctx; ++k) {
-		if (ctx[k]->mi == mi && ctx[k]->d_seq && ctx[k]->d_ki) continue;
-		if (acquire_index(ctx[k], mi) != 0) { fprintf(stderr, "[miniprot_b200] the index is neither resident in a context nor on the host\n"); return -1; }
-	}
-	std::vector<Stages*> st((size_t)n_ctx);
-	for (int32_t k = 0; k < n_ctx; ++k) st[(size_t)k] = ctx[k]->stages;
-	return map_file_multi(st.data(), n_ctx, mi, fn, opt, out);
+	if (fc.hold(mi, false) != 0) return -1;
+	return map_file_multi(fc.st.data(), n_ctx, mi, fn, opt, out);
 }
 
 int32_t mpb_map_file_multi_path(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, const char *out_path)
@@ -786,32 +799,16 @@ int32_t mpb_map_file_multi_path(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_i
 static int32_t map_loci_file_on(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_idx_t *mi, const char *prot_fn, const char *loci_fn, const mp_mapopt_t *opt,
                                 FILE *out, const char *out_path)
 {
-	if (!ctx || n_ctx < 1 || !opt || !mi) return -1;
-	std::vector<mpb_ctx_s*> by_addr(ctx, ctx + n_ctx);
-	std::sort(by_addr.begin(), by_addr.end());
-	if (by_addr[0] == 0 || std::adjacent_find(by_addr.begin(), by_addr.end()) != by_addr.end()) return -1; // a context maps one unit at a time
+	FileCtx fc;
+	if (!fc.distinct(ctx, n_ctx) || !opt || !mi) return -1;
 	LociFile in;
 	int32_t rc = loci_file_read(mi, prot_fn, loci_fn, in);
 	if (rc != 0) return rc;
 	if (bad_scoring(opt->go, opt->ie_coef) || bad_index(mi)) return -3;
 	FILE *fp = out ? out : fopen(out_path, "wb");
 	if (!fp) return -2;
-	{
-		std::vector<std::unique_lock<std::mutex>> held;
-		for (mpb_ctx_s *c : by_addr) held.emplace_back(c->mu); // in address order, as mpb_map_file_multi
-		// the genome is resident in every context before the mappers start (the whole index where a context holds it already)
-		for (int32_t k = 0; k < n_ctx && rc == 0; ++k)
-			if (acquire_genome(ctx[k], mi) != 0) {
-				fprintf(stderr, "[miniprot_b200] the index has no genome on the host and is not resident in the context\n");
-				rc = -1;
-			}
-		std::vector<Stages*> st((size_t)n_ctx);
-		for (int32_t k = 0; k < n_ctx; ++k) st[(size_t)k] = ctx[k]->stages;
-		if (rc == 0) {
-			MPB_CUDA_OK(cudaSetDevice(ctx[0]->device));
-			rc = map_loci_file(st.data(), n_ctx, mi, in, opt, fp);
-		}
-	}
+	rc = fc.hold(mi, true);
+	if (rc == 0) rc = map_loci_file(fc.st.data(), n_ctx, mi, in, opt, fp);
 	if (!out) fclose(fp);
 	return rc;
 }
@@ -849,8 +846,9 @@ mp_reg1_t *mp_map(const mp_idx_t *mi, int qlen, const char *seq, int *n_reg, mp_
 
 int32_t mp_map_file(const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, int)
 {
-	if (CtxPool *p = CtxPool::get()) return mpb_map_file_multi(p->ctx.data(), (int32_t)p->ctx.size(), mi, fn, opt, stdout);
-	return mpb_map_file(mpb_ctx_default(), mi, fn, opt, stdout);
+	CtxPool *p = CtxPool::get();
+	mpb_ctx_s *c = p ? 0 : mpb_ctx_default();
+	return mpb_map_file_multi(p ? p->ctx.data() : &c, p ? (int32_t)p->ctx.size() : 1, mi, fn, opt, stdout);
 }
 
 int64_t mpb_format_paf(const mp_idx_t *mi, const mp_mapopt_t *opt, const char *qname, int32_t qlen, const char *qseq, const mp_reg1_t *r, char **buf,
@@ -1000,14 +998,6 @@ int mpb_sort_segments(mpb_ctx_t *c, int32_t n_seg, const int64_t *off, uint64_t 
 }
 
 void mpb_free(void *p) { free(p); }
-
-void mpb_regs_free(int32_t n, const int32_t *n_reg, mp_reg1_t **reg) // what the caller of mp_map does per protein (map.c:314-318)
-{
-	for (int32_t i = 0; i < n; ++i) {
-		for (int32_t j = 0; j < n_reg[i]; ++j) free(reg[i][j].feat), free(reg[i][j].p);
-		free(reg[i]);
-	}
-}
 
 // CUDA-event bracket on the context's stream (bench.py times its K steps with these); each context has its own pair of events, on
 // its own device

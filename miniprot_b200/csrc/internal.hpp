@@ -110,7 +110,7 @@ struct Stages {
 	virtual void batch_end() {}
 	// wall-clock accounting of the dispatcher's phases (0 S1, 1 H1, 2 S2, 3 H2, 4 S3 waves, 5 H3); optional
 	virtual void note_wall(int /*phase*/, double /*ms*/) {}
-	// called on a host thread before it first calls the stages (the mapper threads of map_file_multi): a device backend makes its
+	// called on a host thread before it first calls the stages (the mapper threads of the file drivers): a device backend makes its
 	// device current there and keeps the thread on the device's NUMA node; optional
 	virtual void thread_init() {}
 	// Locus mode (map_loci).  loci_view(mi, view): until loci_view(0, 0), the stages called with `view` -- an index whose contigs are
@@ -155,9 +155,9 @@ struct LociFile {
 // skipped).  -1 with "file:line: why" on stderr for an unreadable file, a malformed line, an unknown protein or contig, or a bad
 // range; then check_loci()'s -3 refusals; else 0.
 int loci_file_read(const mp_idx_t *mi, const char *prot_fn, const char *loci_fn, LociFile &in);
-// mpb_map_loci_file_multi on n backends: for every pair, in file order, the output of the reference given that locus alone as the
-// genome, in contig coordinates; ids numbered over the whole output.  Returns 0, or -3 (nothing written) for a backend without
-// locus mode.
+// mpb_map_loci_file_multi on n backends (the file driver's pipeline, with map_loci as the mapper): for every pair, in file order, the
+// output of the reference given that locus alone as the genome, in contig coordinates; ids numbered over the whole output.  Returns
+// 0, -1 for n < 1, or -3 (nothing written) for a backend without locus mode.
 int32_t map_loci_file(Stages *const *st, int n, const mp_idx_t *mi, const LociFile &in, const mp_mapopt_t *opt, FILE *out);
 
 // ---------------------------------------------------------------- host pipeline (pipeline.cpp, hits.cpp, align.cpp)
@@ -168,9 +168,15 @@ void map_batch(Stages *st, const mp_idx_t *mi, const mp_mapopt_t *opt, const Bat
 // --dbg-no-refine without -A: the reference aligns regions that have no refined anchors and crashes (mp_align, r->a == NULL).
 // True, with a message on stderr, when mp_dbg_flag and opt ask for that: the callers then map nothing and return -3.
 bool bad_dbg_flags(const mp_mapopt_t *opt);
-int32_t map_file(Stages *st, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, FILE *out);
-// map_file over n backends at once (one mapper thread each); n == 1 is map_file.  The stages must be distinct.
+// The file drivers (map.c:273-343): map_file_multi and map_loci_file run one ordered pipeline over n distinct backends.  One reader
+// thread cuts the input into units of max(1, mini_batch_size / n) residues, one mapper thread per backend (after its thread_init)
+// maps the next unit, and the calling thread writes the units in input order, with one hit-id counter over the whole output.  At
+// most 2n + 1 units are read but not yet written.  With one backend, an input of one unit or MPB_FILE_PIPELINE=0 runs everything on
+// the calling thread.  No thread outlives the call.
+// map_file_multi: a protein FASTA; the QR lines of --dbg-qname carry the index of the backend as tid.  -1 for n < 1 or an input
+// that cannot be opened, -3 for bad_dbg_flags, else 0.  map_file is the same with one backend.
 int32_t map_file_multi(Stages *const *st, int n, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, FILE *out);
+inline int32_t map_file(Stages *st, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, FILE *out) { return map_file_multi(&st, 1, mi, fn, opt, out); }
 
 struct Str {                      // growable output buffer
 	char *s = 0; int64_t l = 0, m = 0;

@@ -321,176 +321,106 @@ static void write_batch(FILE *out, const mp_idx_t *mi, const mp_mapopt_t *opt, c
 	}
 }
 
-// hits are libc-allocated like the reference's (map.c:314-318)
-static void release_regs(const std::vector<int32_t> &n_reg, std::vector<mp_reg1_t*> &reg)
-{
-	for (size_t i = 0; i < reg.size(); ++i) {
-		for (int32_t j = 0; j < n_reg[i]; ++j) free(reg[i][j].feat), free(reg[i][j].p);
-		free(reg[i]);
-	}
-	reg.clear();
-}
+namespace {
 
-// One mini-batch of the query file with everything that must live from the reader to the writer.
-struct FileBatch {
-	std::vector<std::string> names, seqs;
-	std::vector<const char*> sp, np;
-	std::vector<int32_t> len, n_reg;
+// One unit of a file driver's input, with everything that must live from the reader to the writer
+struct Unit {
+	std::vector<std::string> names, seqs; // the records (FASTA input only; the pointers below point into them)
+	std::vector<const char*> sp, np;      // the Batch view
+	std::vector<int32_t> len;
+	const mpb_locus_t *loci = 0;          // locus mode: query q is the protein of pair loci[q]
+	std::vector<int32_t> n_reg;
 	std::vector<mp_reg1_t*> reg;
+	int rc = 0;
 	Batch view() const
 	{
 		Batch b;
-		b.n = (int32_t)seqs.size(), b.seq = sp.data(), b.len = len.data(), b.name = np.data();
+		b.n = (int32_t)len.size(), b.seq = sp.data(), b.len = len.data(), b.name = np.data();
 		return b;
 	}
-	void release() { release_regs(n_reg, reg); }
 };
+typedef std::unique_ptr<Unit> UnitPtr;
 
-// bseq.c:53-74: records until the batch holds mini_batch_size residues; null at the end of the input
-static std::unique_ptr<FileBatch> read_batch(FastxReader &rd, int64_t mini_batch_size, bool &more)
+// bseq.c:53-74: records until the unit holds unit_size residues; null at the end of the input
+UnitPtr read_batch(FastxReader &rd, int64_t unit_size, bool &more)
 {
-	std::unique_ptr<FileBatch> fb(new FileBatch);
+	UnitPtr u(new Unit);
 	std::string name, seq;
 	int64_t residues = 0;
-	while (residues < mini_batch_size && (more = rd.next(name, seq))) {
+	while (residues < unit_size && (more = rd.next(name, seq))) {
 		residues += (int64_t)seq.size();
-		fb->names.push_back(name), fb->seqs.push_back(seq);
+		u->names.push_back(name), u->seqs.push_back(seq);
 	}
-	if (fb->seqs.empty()) return nullptr;
-	const size_t n = fb->seqs.size();
-	fb->sp.resize(n), fb->np.resize(n), fb->len.resize(n), fb->n_reg.assign(n, 0), fb->reg.assign(n, (mp_reg1_t*)0);
-	for (size_t i = 0; i < n; ++i) fb->sp[i] = fb->seqs[i].c_str(), fb->np[i] = fb->names[i].c_str(), fb->len[i] = (int32_t)fb->seqs[i].size();
-	return fb;
+	if (u->seqs.empty()) return nullptr;
+	const size_t n = u->seqs.size();
+	for (size_t i = 0; i < n; ++i) u->sp.push_back(u->seqs[i].c_str()), u->np.push_back(u->names[i].c_str()), u->len.push_back((int32_t)u->seqs[i].size());
+	u->n_reg.assign(n, 0), u->reg.assign(n, (mp_reg1_t*)0);
+	return u;
 }
 
-// A one-slot hand-over between two steps of the file pipeline: put() waits while the slot is taken, take() returns null once
-// the producer has closed an empty slot.
-class Handoff {
-public:
-	void put(std::unique_ptr<FileBatch> fb)
-	{
-		std::unique_lock<std::mutex> lk(mu_);
-		cv_.wait(lk, [&] { return !slot_; });
-		slot_ = std::move(fb);
-		cv_.notify_all();
-	}
-	void close()
-	{
-		std::lock_guard<std::mutex> lk(mu_);
-		closed_ = true;
-		cv_.notify_all();
-	}
-	std::unique_ptr<FileBatch> take()
-	{
-		std::unique_lock<std::mutex> lk(mu_);
-		cv_.wait(lk, [&] { return slot_ || closed_; });
-		std::unique_ptr<FileBatch> fb = std::move(slot_);
-		cv_.notify_all();
-		return fb;
-	}
-
-private:
-	std::mutex mu_;
-	std::condition_variable cv_;
-	std::unique_ptr<FileBatch> slot_;
-	bool closed_ = false;
-};
-
-// map.c:273-343 (worker_pipeline under kt_pipeline with three steps): step 0 reads and parses the next mini-batch, step 1 maps
-// it (the GPU batch dispatcher above), step 2 formats and writes the hits -- in the order of the input, by one thread, which
-// also owns the hit counter.  As in the reference, step 0 of batch n+1 and step 2 of batch n-1 run while batch n is mapped:
-// one reader thread, the calling thread as the mapper (it owns the device), one writer thread, a one-slot hand-over between
-// neighbours.  An input that fits one mini-batch has nothing to overlap and starts no thread; MPB_FILE_PIPELINE=0 runs the three
-// steps one after another on the calling thread for any input (A/B, debugging).
-int32_t map_file(Stages *st, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, FILE *out)
+// map.c:273-343 (worker_pipeline under kt_pipeline with three steps), over n backends: one reader thread cuts the input into units
+// (read(more) returns the next unit, or null at the end, and clears `more` once the input is exhausted), one mapper thread per backend
+// maps the next unit each (map(st[k], k, unit)), and the calling thread writes the units strictly in input order and owns the hit
+// counter.  At most 2n + 1 units are read but not yet written: with one backend, reading unit k+1 and writing unit k-1 overlap the
+// mapping of unit k, as in the reference.  The host phases of the mappers share one worker pool and take turns on it (parfor.hpp);
+// the device stages overlap.  With one backend, an input that fits one unit has nothing to overlap and starts no thread, and
+// MPB_FILE_PIPELINE=0 runs the three steps one after another on the calling thread for any input (A/B, debugging).  Returns the first
+// non-zero return code of a unit, else 0.
+template <class Read, class Map>
+int32_t run_units(Stages *const *st, int n, const mp_idx_t *mi, const mp_mapopt_t *opt, FILE *out, const char *label, const char *noun, Read read, Map map)
 {
-	if (bad_dbg_flags(opt)) return -3;
-	FastxReader rd(fn);
-	if (!rd.fp) return -1;
+	if (opt->flag & MP_F_GFF) fputs("##gff-version 3\n", out); // map.c:338
+	static const bool trace = getenv("MPB_TRACE") != 0;
 	int64_t id_counter = 0;
-	if (opt->flag & MP_F_GFF) fputs("##gff-version 3\n", out); // map.c:338
-	auto map_step = [&](FileBatch &fb) {
-		map_batch(st, mi, opt, fb.view(), fb.n_reg.data(), fb.reg.data(), 0);
-		if (mp_verbose >= 3)
-			fprintf(stderr, "[M::%s::%.3f*%.2f] mapped %d sequences\n", "map_file", mp_realtime(), mp_cputime() / mp_realtime(), (int)fb.seqs.size());
+	int32_t rc = 0;
+	auto map_step = [&](int k, Unit &u) {
+		map(st[k], k, u);
+		if (mp_verbose < 3) return;
+		if (n > 1) fprintf(stderr, "[M::%s::%.3f*%.2f] mapped %d %s (context %d)\n", label, mp_realtime(), mp_cputime() / mp_realtime(), (int)u.len.size(), noun, k);
+		else fprintf(stderr, "[M::%s::%.3f*%.2f] mapped %d %s\n", label, mp_realtime(), mp_cputime() / mp_realtime(), (int)u.len.size(), noun);
 	};
-	static const bool trace = getenv("MPB_TRACE") != 0;
-	auto write_step = [&](FileBatch &fb) {
+	auto write_step = [&](int64_t i, Unit &u) {
+		if (u.rc != 0 && rc == 0) rc = u.rc;
 		const double t0 = mp_realtime();
-		write_batch(out, mi, opt, fb.view(), fb.n_reg.data(), fb.reg.data(), &id_counter);
+		write_batch(out, mi, opt, u.view(), u.n_reg.data(), u.reg.data(), &id_counter, u.loci);
 		const double t1 = mp_realtime();
-		fb.release();
-		if (trace) fprintf(stderr, "[mpb-trace] output: %d proteins formatted + written in %.2f ms, released in %.2f ms\n", (int)fb.seqs.size(), (t1 - t0) * 1e3, (mp_realtime() - t1) * 1e3);
+		mpb_regs_free((int32_t)u.reg.size(), u.n_reg.data(), u.reg.data());
+		if (trace)
+			fprintf(stderr, "[mpb-trace] output: unit %ld, %d %s formatted + written in %.2f ms, released in %.2f ms\n", (long)i, (int)u.len.size(), noun, (t1 - t0) * 1e3,
+			        (mp_realtime() - t1) * 1e3);
 	};
-	const char *e = getenv("MPB_FILE_PIPELINE");
 	bool more = true;
-	std::unique_ptr<FileBatch> first = read_batch(rd, opt->mini_batch_size, more);
+	UnitPtr first = read(more);
 	if (!first) return 0;
-	if ((e && atoi(e) == 0) || !more) { // the whole input is one mini-batch (nothing to overlap: no threads), or the serial form was asked for
-		for (std::unique_ptr<FileBatch> fb = std::move(first); fb; fb = more ? read_batch(rd, opt->mini_batch_size, more) : std::unique_ptr<FileBatch>()) {
-			map_step(*fb);
-			write_step(*fb);
+	const char *e = getenv("MPB_FILE_PIPELINE");
+	if (n == 1 && (!more || (e && atoi(e) == 0))) {
+		int64_t i = 0;
+		for (UnitPtr u = std::move(first); u; u = more ? read(more) : nullptr) {
+			map_step(0, *u);
+			write_step(i++, *u);
 		}
-		return 0;
+		return rc;
 	}
-	Handoff to_map, to_write;
-	std::thread reader([&] {
-		while (more) {
-			std::unique_ptr<FileBatch> fb = read_batch(rd, opt->mini_batch_size, more);
-			if (!fb) break;
-			to_map.put(std::move(fb));
-		}
-		to_map.close();
-	});
-	std::thread writer([&] {
-		while (std::unique_ptr<FileBatch> fb = to_write.take()) write_step(*fb);
-	});
-	for (std::unique_ptr<FileBatch> fb = std::move(first); fb; fb = to_map.take()) {
-		map_step(*fb);
-		to_write.put(std::move(fb));
-	}
-	to_write.close();
-	reader.join();
-	writer.join();
-	return 0;
-}
 
-// map_file over n backends (contexts, possibly on several devices): one reader thread cuts the input into work units of at most
-// mini_batch_size / n residues (at least one protein; results do not depend on batch boundaries), n mapper threads -- one per
-// backend -- take the next unit each, and one writer thread emits the units strictly in input order and owns the hit counter, as
-// in map_file.  At most 2n units are between the reader and the writer, so memory stays bounded whatever the input.
-// The host phases of the mappers share one worker pool and take turns on it (parfor.hpp), the device stages overlap.
-int32_t map_file_multi(Stages *const *st, int n, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, FILE *out)
-{
-	if (n < 1) return -1;
-	if (n == 1) return map_file(st[0], mi, fn, opt, out);
-	if (bad_dbg_flags(opt)) return -3;
-	FastxReader rd(fn);
-	if (!rd.fp) return -1;
-	if (opt->flag & MP_F_GFF) fputs("##gff-version 3\n", out); // map.c:338
-	const int64_t unit_size = std::max<int64_t>(1, opt->mini_batch_size / n);
-	const int64_t max_in_flight = 2 * (int64_t)n;
-	static const bool trace = getenv("MPB_TRACE") != 0;
-
+	const int64_t max_in_flight = 2 * (int64_t)n + 1;
 	std::mutex mu;
 	std::condition_variable cv;
-	std::deque<std::pair<int64_t, std::unique_ptr<FileBatch>>> todo; // read, not yet taken by a mapper
-	std::map<int64_t, std::unique_ptr<FileBatch>> mapped;              // mapped, not yet written
-	int64_t n_read = 0, n_written = 0;                                   // units
-	bool eof = false;
-
+	std::deque<std::pair<int64_t, UnitPtr>> todo; // read, not yet taken by a mapper
+	std::map<int64_t, UnitPtr> mapped;              // mapped, not yet written
+	int64_t n_read = 1, n_written = 0;              // units
+	bool eof = !more;
+	todo.emplace_back(0, std::move(first));
 	std::thread reader([&] {
-		bool more = true;
-		while (more) {
+		for (bool last = eof; !last;) {
 			{
 				std::unique_lock<std::mutex> lk(mu);
 				cv.wait(lk, [&] { return n_read - n_written < max_in_flight; });
 			}
-			std::unique_ptr<FileBatch> fb = read_batch(rd, unit_size, more);
-			const bool last = !fb || !more;
+			UnitPtr u = read(more);
+			last = !u || !more;
 			std::lock_guard<std::mutex> lk(mu);
-			if (fb) todo.emplace_back(n_read++, std::move(fb));
-			if (last) eof = true;
+			if (u) todo.emplace_back(n_read++, std::move(u));
+			eof = last;
 			cv.notify_all();
 		}
 	});
@@ -499,7 +429,7 @@ int32_t map_file_multi(Stages *const *st, int n, const mp_idx_t *mi, const char 
 		mappers.emplace_back([&, k] {
 			st[k]->thread_init();
 			for (;;) {
-				std::pair<int64_t, std::unique_ptr<FileBatch>> u;
+				std::pair<int64_t, UnitPtr> u;
 				{
 					std::unique_lock<std::mutex> lk(mu);
 					cv.wait(lk, [&] { return !todo.empty() || eof; });
@@ -507,40 +437,44 @@ int32_t map_file_multi(Stages *const *st, int n, const mp_idx_t *mi, const char 
 					u = std::move(todo.front());
 					todo.pop_front();
 				}
-				FileBatch &fb = *u.second;
-				map_batch(st[k], mi, opt, fb.view(), fb.n_reg.data(), fb.reg.data(), k);
-				if (mp_verbose >= 3)
-					fprintf(stderr, "[M::%s::%.3f*%.2f] mapped %d sequences (context %d)\n", "map_file_multi", mp_realtime(), mp_cputime() / mp_realtime(), (int)fb.seqs.size(), k);
+				map_step(k, *u.second);
 				std::lock_guard<std::mutex> lk(mu);
 				mapped.emplace(u.first, std::move(u.second));
 				cv.notify_all();
 			}
 		});
-	std::thread writer([&] {
-		int64_t id_counter = 0;
-		for (;;) {
-			std::unique_ptr<FileBatch> fb;
-			{
-				std::unique_lock<std::mutex> lk(mu);
-				cv.wait(lk, [&] { return mapped.count(n_written) || (eof && n_written == n_read); });
-				auto it = mapped.find(n_written);
-				if (it == mapped.end()) return; // everything read has been written
-				fb = std::move(it->second);
-				mapped.erase(it);
-			}
-			const double t0 = mp_realtime();
-			write_batch(out, mi, opt, fb->view(), fb->n_reg.data(), fb->reg.data(), &id_counter);
-			fb->release();
-			if (trace) fprintf(stderr, "[mpb-trace] output: unit %ld, %d proteins formatted + written in %.2f ms\n", (long)n_written, (int)fb->seqs.size(), (mp_realtime() - t0) * 1e3);
-			std::lock_guard<std::mutex> lk(mu);
-			++n_written;
-			cv.notify_all();
+	for (int64_t i = 0;; ++i) {
+		UnitPtr u;
+		{
+			std::unique_lock<std::mutex> lk(mu);
+			cv.wait(lk, [&] { return mapped.count(i) || (eof && i == n_read); });
+			auto it = mapped.find(i);
+			if (it == mapped.end()) break; // everything read has been written
+			u = std::move(it->second);
+			mapped.erase(it);
 		}
-	});
+		write_step(i, *u);
+		u.reset();
+		std::lock_guard<std::mutex> lk(mu);
+		n_written = i + 1;
+		cv.notify_all();
+	}
 	reader.join();
 	for (std::thread &t : mappers) t.join();
-	writer.join();
-	return 0;
+	return rc;
+}
+
+} // namespace
+
+int32_t map_file_multi(Stages *const *st, int n, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, FILE *out)
+{
+	if (n < 1) return -1;
+	if (bad_dbg_flags(opt)) return -3;
+	FastxReader rd(fn);
+	if (!rd.fp) return -1;
+	const int64_t unit_size = std::max<int64_t>(1, opt->mini_batch_size / n);
+	return run_units(st, n, mi, opt, out, "map_file", "sequences", [&](bool &more) { return read_batch(rd, unit_size, more); },
+	                 [&](Stages *s, int k, Unit &u) { map_batch(s, mi, opt, u.view(), u.n_reg.data(), u.reg.data(), k); });
 }
 
 // ---------------------------------------------------------------- locus mode
@@ -724,24 +658,8 @@ int loci_file_read(const mp_idx_t *mi, const char *prot_fn, const char *loci_fn,
 	return check_loci(mi, (int32_t)in.seqs.size(), (int32_t)in.loci.size(), in.loci.data());
 }
 
-namespace {
-
-// pairs [i0, i0 + n) of a loci file and their hits, from the mapper that aligned them to the writer
-struct LociUnit {
-	int32_t i0 = 0, n = 0;
-	std::vector<int32_t> n_reg;
-	std::vector<mp_reg1_t*> reg;
-	int rc = 0;
-	void release() { release_regs(n_reg, reg); }
-};
-
-} // namespace
-
-// map_file_multi's pipeline over the pairs of a loci file, which are in memory already: the pairs are cut into units of at most
-// mini_batch_size / n residues (at least one pair), n mapper threads -- one per backend -- take the next unit each and align it
-// with map_loci, and the calling thread writes the units in input order and owns the hit counter.  At most 2n units are between
-// the mappers and the writer.  With one backend, a single unit or MPB_FILE_PIPELINE=0 (one backend) runs everything on the
-// calling thread.  Hits do not depend on unit boundaries (map_loci), so neither does the output.
+// run_units over the pairs of a loci file, which are in memory already: units of at most mini_batch_size / n residues (at least one
+// pair), each aligned with map_loci.  Hits do not depend on unit boundaries (map_loci), so neither does the output.
 int32_t map_loci_file(Stages *const *st, int n, const mp_idx_t *mi, const LociFile &in, const mp_mapopt_t *opt, FILE *out)
 {
 	if (n < 1) return -1;
@@ -752,77 +670,34 @@ int32_t map_loci_file(Stages *const *st, int n, const mp_idx_t *mi, const LociFi
 		}
 	const int32_t n_loci = (int32_t)in.loci.size();
 	const int64_t unit_size = std::max<int64_t>(1, opt->mini_batch_size / n);
-	std::vector<std::unique_ptr<LociUnit>> units;
-	for (int32_t i0 = 0; i0 < n_loci;) {
-		int32_t i1 = i0;
-		for (int64_t residues = 0; i1 < n_loci && residues < unit_size; ++i1) residues += in.len[(size_t)in.loci[(size_t)i1].qid];
-		units.emplace_back(new LociUnit);
-		units.back()->i0 = i0, units.back()->n = i1 - i0;
-		i0 = i1;
-	}
-	if (opt->flag & MP_F_GFF) fputs("##gff-version 3\n", out); // map.c:338
-	auto map_step = [&](Stages *s, LociUnit &u) {
-		u.n_reg.assign((size_t)u.n, 0), u.reg.assign((size_t)u.n, (mp_reg1_t*)0);
-		u.rc = map_loci(s, mi, opt, (int32_t)in.seqs.size(), in.sp.data(), in.len.data(), in.np.data(), u.n, in.loci.data() + u.i0, u.n_reg.data(), u.reg.data());
-	};
-	int64_t id_counter = 0;
-	int32_t rc = 0;
-	auto write_step = [&](LociUnit &u) {
-		if (u.rc != 0 && rc == 0) rc = u.rc;
-		std::vector<const char*> sp((size_t)u.n), np((size_t)u.n);
-		std::vector<int32_t> lp((size_t)u.n);
-		for (int32_t k = 0; k < u.n; ++k) {
-			const int32_t q = in.loci[(size_t)(u.i0 + k)].qid;
-			sp[(size_t)k] = in.sp[(size_t)q], np[(size_t)k] = in.np[(size_t)q], lp[(size_t)k] = in.len[(size_t)q];
-		}
-		Batch b;
-		b.n = u.n, b.seq = sp.data(), b.len = lp.data(), b.name = np.data();
-		write_batch(out, mi, opt, b, u.n_reg.data(), u.reg.data(), &id_counter, in.loci.data() + u.i0);
-		u.release();
-	};
-	const char *e = getenv("MPB_FILE_PIPELINE");
-	if (n == 1 && ((e && atoi(e) == 0) || units.size() <= 1)) {
-		for (std::unique_ptr<LociUnit> &u : units) map_step(st[0], *u), write_step(*u), u.reset();
-		return rc;
-	}
-	const size_t max_in_flight = 2 * (size_t)n;
-	std::mutex mu;
-	std::condition_variable cv;
-	size_t n_taken = 0, n_written = 0;
-	std::vector<char> mapped(units.size(), 0);
-	std::vector<std::thread> mappers;
-	for (int k = 0; k < n; ++k)
-		mappers.emplace_back([&, k] {
-			st[k]->thread_init();
-			for (;;) {
-				size_t u;
-				{
-					std::unique_lock<std::mutex> lk(mu);
-					cv.wait(lk, [&] { return n_taken == units.size() || n_taken - n_written < max_in_flight; });
-					if (n_taken == units.size()) return;
-					u = n_taken++;
-				}
-				map_step(st[k], *units[u]);
-				if (mp_verbose >= 3)
-					fprintf(stderr, "[M::%s::%.3f*%.2f] aligned %d pairs (context %d)\n", "map_loci_file", mp_realtime(), mp_cputime() / mp_realtime(), units[u]->n, k);
-				std::lock_guard<std::mutex> lk(mu);
-				mapped[u] = 1;
-				cv.notify_all();
+	int32_t i0 = 0;
+	auto read = [&](bool &more) {
+		UnitPtr u;
+		if (i0 < n_loci) {
+			u.reset(new Unit);
+			u->loci = in.loci.data() + i0;
+			for (int64_t residues = 0; i0 < n_loci && residues < unit_size; ++i0) {
+				const size_t q = (size_t)in.loci[(size_t)i0].qid;
+				residues += in.len[q];
+				u->sp.push_back(in.sp[q]), u->np.push_back(in.np[q]), u->len.push_back(in.len[q]);
 			}
-		});
-	for (size_t w = 0; w < units.size(); ++w) {
-		{
-			std::unique_lock<std::mutex> lk(mu);
-			cv.wait(lk, [&] { return mapped[w] != 0; });
+			u->n_reg.assign(u->len.size(), 0), u->reg.assign(u->len.size(), (mp_reg1_t*)0);
 		}
-		write_step(*units[w]);
-		units[w].reset();
-		std::lock_guard<std::mutex> lk(mu);
-		++n_written;
-		cv.notify_all();
-	}
-	for (std::thread &t : mappers) t.join();
-	return rc;
+		more = i0 < n_loci;
+		return u;
+	};
+	return run_units(st, n, mi, opt, out, "map_loci_file", "pairs", read, [&](Stages *s, int, Unit &u) {
+		u.rc = map_loci(s, mi, opt, (int32_t)in.seqs.size(), in.sp.data(), in.len.data(), in.np.data(), (int32_t)u.len.size(), u.loci, u.n_reg.data(), u.reg.data());
+	});
 }
 
 } // namespace mpb
+
+// what the caller of mp_map does per protein (map.c:314-318): the hits are libc-allocated like the reference's
+void mpb_regs_free(int32_t n, const int32_t *n_reg, mp_reg1_t **reg)
+{
+	for (int32_t i = 0; i < n; ++i) {
+		for (int32_t j = 0; j < n_reg[i]; ++j) free(reg[i][j].feat), free(reg[i][j].p);
+		free(reg[i]);
+	}
+}

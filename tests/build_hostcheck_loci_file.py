@@ -10,6 +10,8 @@ OUT = os.path.join(ROOT, "tests", "_build", "loci_file", "libhostcheck_loci_file
 
 
 def build(force=False):
+    if os.environ.get("MPB_HOSTCHECK_LOCI_FILE_SO"):  # a build made elsewhere, e.g. with -fsanitize=thread (run python under LD_PRELOAD=libtsan)
+        return os.environ["MPB_HOSTCHECK_LOCI_FILE_SO"]
     hc = os.path.join(ROOT, "tests", "hostcheck")
     srcs = [os.path.join(CSRC, s) for s in HOST_SRCS] + [os.path.join(hc, "hostcheck_loci_file.cpp")]
     ora = sorted(glob.glob(os.path.join(ROOT, "oracle", "*.c")))

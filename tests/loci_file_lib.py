@@ -31,6 +31,7 @@ OPTION_SETS = {
     "gff": ["--gff"],
     "gff_only_P": ["--gff-only", "-P", "XY"],
     "gtf": ["--gtf"],
+    "gtf_unmapped": ["--gtf", "-u"],
     "aln": ["--aln"],
     "trans_gff": ["--trans", "--gff"],
     "unmapped_outn1": ["-u", "--outn=1"],

@@ -1,6 +1,6 @@
-"""CPU: the multi-context file driver (map_file_multi: one reader, n mapper threads, one writer in input order) with n independent
-oracle backends writes what the one-context driver writes, byte for byte, in every output format -- also when the work units
-finish out of input order (HC_UNIT_DELAY) and when a unit holds a single protein."""
+"""CPU: the file driver (map_file: one reader, n mapper threads, the calling thread writing in input order) with n independent oracle
+backends writes the reference's output, byte for byte, in every output format, for one backend as for several -- also when the work
+units finish out of input order (HC_UNIT_DELAY) and when a unit holds a single protein."""
 import ctypes as C
 import gzip
 import os
@@ -45,9 +45,9 @@ def run(hc, g, p, out, n, flag=0, mini_batch=0):
 
 @pytest.mark.parametrize("pipeline", ["1", "0"])
 @pytest.mark.parametrize("mini_batch", [0, 1200, 1])
-@pytest.mark.parametrize("n", [2, 3, 5])
+@pytest.mark.parametrize("n", [1, 2, 3, 5])
 def test_paf_golden(hc, sets, tmp_path, monkeypatch, n, mini_batch, pipeline):
-    """MPB_FILE_PIPELINE=0 (the serial form of the one-context driver) must not change what the multi-context driver does."""
+    """MPB_FILE_PIPELINE=0 (the serial form, with one backend only) must not change the output."""
     monkeypatch.setenv("HC_UNIT_DELAY", str(7 * n + mini_batch))
     monkeypatch.setenv("MPB_FILE_PIPELINE", pipeline)
     for name, paf in (("tiny", "tiny.paf"), ("tiny5", "tiny5.paf")):
@@ -55,7 +55,7 @@ def test_paf_golden(hc, sets, tmp_path, monkeypatch, n, mini_batch, pipeline):
         assert run(hc, g, p, str(tmp_path / "o.paf"), n, mini_batch=mini_batch) == gold(paf), name
 
 
-@pytest.mark.parametrize("n", [2, 3, 5])
+@pytest.mark.parametrize("n", [1, 2, 3, 5])
 def test_dpp3_paf_golden(hc, sets, tmp_path, monkeypatch, n):
     """The reference's DPP3 pair (the oracle DP is slow on it: one mini-batch size per mapper count)."""
     monkeypatch.setenv("HC_UNIT_DELAY", str(n))
@@ -67,7 +67,7 @@ FORMATS = {"gff": (0x8, None), "gtf": (0x20, None), "aln": (0x80, None), "trans"
 
 
 @pytest.mark.parametrize("fmt", sorted(FORMATS))
-@pytest.mark.parametrize("n", [2, 3, 5])
+@pytest.mark.parametrize("n", [1, 2, 3, 5])
 def test_other_formats_golden(hc, sets, tmp_path, monkeypatch, n, fmt):
     """GFF3 / GTF number every printed hit with a counter that runs over the whole file: units mapped out of order must not
     disturb it."""
@@ -98,6 +98,8 @@ lib = C.CDLL(sys.argv[1])
 lib.hc_map_file_multi.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_uint32, C.c_int64, C.c_int32]
 g, p, empty, out = (a.encode() for a in sys.argv[2:6])
 assert lib.hc_map_file_multi(g, p, out, 0, 1, 4) == 0
+assert lib.hc_map_file_multi(g, p, out, 0, 1, 1) == 0  # one mapper thread
+assert lib.hc_map_file_multi(g, p, out, 0, 0, 1) == 0  # one unit: no thread
 assert lib.hc_map_file_multi(g, empty, out, 0, 0, 4) == 0
 assert lib.hc_map_file_multi(g, b"/nonexistent.faa", out, 0, 0, 4) == -1
 assert threading.active_count() == 1
