@@ -387,7 +387,28 @@ typedef struct {
 	double ms_prep;    /* row preparation kernels */
 } mpb_stats_t;
 void mpb_get_stats(const mpb_ctx_t *ctx, mpb_stats_t *st);
-void mpb_reset_stats(mpb_ctx_t *ctx);
+void mpb_reset_stats(mpb_ctx_t *ctx); /* also resets the counters of mpb_get_mem_stats(); the peak restarts at what is held */
+
+/* Device memory.  The working arenas of a context -- every device buffer it holds except the resident index and the --spsc table --
+ * may hold at most `bytes` at once; 0 (the default) is automatic: what they hold plus the device's free memory less a sixteenth of the device (at least 1 GiB), asked of
+ * the device only when an arena has to grow.  The seeding, refinement and DP stages run a batch in consecutive slices of proteins,
+ * locus pairs, windows and DP problems whose arenas fit, and idle arenas of the other stages are released, largest first, when
+ * one has to grow past the allowance.  Results do not depend on the budget.  A single item that does not fit on its own runs alone
+ * anyway (n_over_budget), and may still fail to allocate.  Applies from the next call; idle arenas above a new budget are released
+ * at once.  Returns 0, or -1 for a null context or a negative value.  MPB_DEVICE_MEM=<n>[k|m|g], read when a context is created,
+ * sets the budget of every context, the default one included (an invalid value is reported and leaves automatic mode). */
+int mpb_ctx_set_mem_budget(mpb_ctx_t *ctx, int64_t bytes);
+typedef struct {
+	int64_t budget;         /* bytes, 0 = automatic */
+	int64_t allowance;      /* the last allowance computed (the budget, or what automatic mode found) */
+	int64_t held, peak_held; /* bytes the working arenas hold, and the most they held at once */
+	int64_t n_slices_seed, n_slices_loci, n_slices_refine; /* slices of the seeding (whole genome, locus mode) and refinement stages */
+	int64_t n_subwaves;     /* sub-waves of the DP stage */
+	int64_t n_released, bytes_released; /* arenas released to make room, and their bytes */
+	int64_t n_over_budget;  /* items that ran alone above the allowance, and any other growth of an arena past it: while this is 0,
+	                         * peak_held stays within an explicit budget */
+} mpb_mem_stats_t;
+void mpb_get_mem_stats(const mpb_ctx_t *ctx, mpb_mem_stats_t *st);
 
 #ifdef __cplusplus
 }

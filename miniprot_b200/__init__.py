@@ -128,6 +128,11 @@ class Stats(C.Structure):  # mpb_stats_t
                 ("ms_bt", C.c_double), ("ms_dp_wave", C.c_double), ("ms_prep", C.c_double)]
 
 
+class MemStats(C.Structure):  # mpb_mem_stats_t
+    _fields_ = [(f, C.c_int64) for f in ("budget", "allowance", "held", "peak_held", "n_slices_seed", "n_slices_loci", "n_slices_refine",
+                                         "n_subwaves", "n_released", "bytes_released", "n_over_budget")]
+
+
 class Extra(C.Structure):  # mp_extra_t without its trailing cigar[]
     _fields_ = [(f, C.c_int32) for f in ("dp_score", "dp_max", "dp_max2", "n_cigar", "m_cigar", "blen", "n_fs", "n_stop", "dist_stop",
                                          "dist_start", "n_iden", "n_plus")]
@@ -230,6 +235,9 @@ def lib() -> C.CDLL:
                                       C.POINTER(C.c_void_p), C.c_void_p, C.POINTER(C.c_void_p)]
         L.mpb_get_stats.argtypes = [C.c_void_p, C.POINTER(Stats)]
         L.mpb_reset_stats.argtypes = [C.c_void_p]
+        L.mpb_ctx_set_mem_budget.restype = C.c_int
+        L.mpb_ctx_set_mem_budget.argtypes = [C.c_void_p, C.c_int64]
+        L.mpb_get_mem_stats.argtypes = [C.c_void_p, C.POINTER(MemStats)]
         L.mpb_free.argtypes = [C.c_void_p]
         L.mp_mapopt_set_max_intron.argtypes = [C.POINTER(MapOpt), C.c_int64]
         L.mp_start()
@@ -277,7 +285,18 @@ class Context:
         return s
 
     def reset_stats(self):
+        """Reset the counters of stats() and mem_stats() (the peak restarts at what the arenas hold)."""
         lib().mpb_reset_stats(self.h)
+
+    def set_mem_budget(self, nbytes: int) -> int:
+        """Cap the bytes the context's working arenas may hold at once (0: automatic, what the device has free less a sixteenth of it, at least 1 GiB).
+        Stages then run in slices that fit; results do not change.  Returns 0, or -1 for a negative value."""
+        return lib().mpb_ctx_set_mem_budget(self.h, nbytes)
+
+    def mem_stats(self) -> MemStats:
+        s = MemStats()
+        lib().mpb_get_mem_stats(self.h, C.byref(s))
+        return s
 
 
 def idxopt() -> IdxOpt:

@@ -9,6 +9,7 @@
 #include "stages_dev.hpp"
 #include "seed_dev.hpp"
 #include "../align.hpp"
+#include "../slices.hpp"
 
 using namespace mpb;
 using namespace mpb::cuda;
@@ -133,13 +134,20 @@ struct CudaStages : Stages {
 		ctx->stats.h2d_bytes += (int64_t)tot;
 		return ctx->b_aa.as<char>();
 	}
+	// (the residues stay resident from batch_begin to batch_end: the ledger does not release them between the stages)
+	bool aa_held = false;
 	void batch_begin(const Batch &b) override
 	{
 		cur_batch = 0;
 		upload_residues(b, cur_off);
 		cur_batch = &b;
+		if (!aa_held) ++ctx->b_aa.busy, aa_held = true;
 	}
-	void batch_end() override { cur_batch = 0; }
+	void batch_end() override
+	{
+		cur_batch = 0;
+		if (aa_held) --ctx->b_aa.busy, aa_held = false;
+	}
 
 	void note_wall(int phase, double ms) override { if (phase >= 0 && phase < 6) ctx->stats.ms_wall[phase] += ms; }
 	void seed_chain(const mp_idx_t *mi, const mp_mapopt_t *opt, const Batch &b, ChainSet &out) override
@@ -170,6 +178,7 @@ struct CudaStages : Stages {
 		const char *d_aa = upload_residues(b, off);
 		std::vector<DpDev> dj(jobs.size());
 		for (size_t k = 0; k < jobs.size(); ++k) dj[k] = make_dev_job(mi, jobs[k], off[(size_t)jobs[k].qid]);
+		Busy busy({ &ctx->b_aa });
 		if (mi->nt->spsc && ctx->ss_src != mi->nt->spsc) build_spsc_table(ctx, mi);
 		nasw_run(ctx, ctx->d_seq, mi->nt->spsc ? ctx->d_ss : 0, d_aa, base, dj, out);
 	}
@@ -309,6 +318,16 @@ mpb_ctx_s *ctx_new(int device, bool pin)
 	MPB_CUDA_OK(cudaEventCreate(&c->ev_w1));
 	MPB_CUDA_OK(cudaEventCreate(&c->ev_p0));
 	memset(&c->stats, 0, sizeof(c->stats));
+	c->mem.device = device;
+	for (DevBuf *b : { &c->b_jobs, &c->b_order, &c->b_chunks, &c->b_rw, &c->b_aa, &c->b_out, &c->b_carry, &c->b_tb, &c->b_cigar, &c->b_cigpack, &c->b_cigoff,
+	                   &c->b_packed, &c->b_units })
+		c->mem.add(*b);
+	for (DevBuf &b : c->b_c) c->mem.add(b);
+	if (const char *e = getenv("MPB_DEVICE_MEM")) {
+		const int64_t v = parse_mem_size(e);
+		if (v < 0) fprintf(stderr, "[miniprot_b200] MPB_DEVICE_MEM=%s: expected <bytes>[k|m|g]; the device-memory budget stays automatic\n", e);
+		else c->mem.budget = v;
+	}
 	c->stages = new CudaStages(c);
 	{
 		std::lock_guard<std::mutex> lk(g_default_mu);
@@ -605,6 +624,7 @@ static int build_index_on_device(mp_idx_t *mi)
 	const double t0 = mp_realtime();
 	forget_adopters(c);
 	if (c->own_index) forget_index(c); // the build reuses the context's own buffers
+	Busy busy(c->b_c, 16);
 	if (idx_build_device(c, mi) != 0) return -1;
 	c->d_ki = c->own_ki.as<int64_t>(), c->d_kb = c->own_kb.as<uint32_t>(), c->d_seq = c->own_seq.as<uint8_t>();
 	upload_meta(c, mi);
@@ -893,6 +913,7 @@ int mpb_nasw_batch(mpb_ctx_t *c, const ns_opt_t *opt, int32_t n, const mpb_dp_pr
 		if (p.ss) memcpy(ssb.data() + g, p.ss, (size_t)p.nl), d.ss_off = 0; // splice bytes travel laid out like the packed bases
 		g += p.nl + 2, a += p.al;
 	}
+	Busy busy({ &c->b_packed, &c->b_aa, &c->b_c[15] });
 	c->b_packed.reserve(packed.size() + 16);
 	c->b_aa.reserve(aa.size() + 16);
 	MPB_CUDA_OK(cudaMemcpyAsync(c->b_packed.p, packed.data(), packed.size(), cudaMemcpyHostToDevice, c->stream));
@@ -988,6 +1009,7 @@ int mpb_sort_segments(mpb_ctx_t *c, int32_t n_seg, const int64_t *off, uint64_t 
 	MPB_CUDA_OK(cudaSetDevice(c->device));
 	const size_t N = n_seg ? (size_t)off[n_seg] : 0;
 	if (N == 0) return 0;
+	Busy busy({ &c->b_c[1], &c->b_c[2], &c->b_c[3] });
 	c->b_c[1].reserve(sizeof(uint64_t) * (N + 2)), c->b_c[2].reserve(sizeof(uint64_t) * (N + 2));
 	MPB_CUDA_OK(cudaMemcpyAsync(c->b_c[1].p, keys, sizeof(uint64_t) * N, cudaMemcpyHostToDevice, c->stream));
 	seg_sort_u64(c, c->stream, c->b_c[1].as<uint64_t>(), c->b_c[2].as<uint64_t>(), n_seg, off, off + 1);
@@ -1045,6 +1067,29 @@ void mpb_reset_stats(mpb_ctx_t *c)
 {
 	std::lock_guard<std::mutex> cl(c->mu);
 	memset(&c->stats, 0, sizeof(c->stats));
+	c->mem.reset_counters();
+}
+
+int mpb_ctx_set_mem_budget(mpb_ctx_t *c, int64_t bytes)
+{
+	if (!c || bytes < 0) return -1;
+	std::lock_guard<std::mutex> cl(c->mu);
+	c->mem.budget = bytes;
+	if (bytes > 0 && c->mem.held > bytes) { // between calls no arena is in use
+		MPB_CUDA_OK(cudaSetDevice(c->device));
+		MPB_CUDA_OK(cudaStreamSynchronize(c->stream));
+		c->mem.release_idle(bytes, 0);
+	}
+	return 0;
+}
+
+void mpb_get_mem_stats(const mpb_ctx_t *c, mpb_mem_stats_t *st)
+{
+	std::lock_guard<std::mutex> cl(c->mu);
+	const Ledger &m = c->mem;
+	st->budget = m.budget, st->allowance = m.allowance_last, st->held = m.held, st->peak_held = m.peak;
+	st->n_slices_seed = m.n_slices_seed, st->n_slices_loci = m.n_slices_loci, st->n_slices_refine = m.n_slices_refine, st->n_subwaves = m.n_subwaves;
+	st->n_released = m.n_released, st->bytes_released = m.bytes_released, st->n_over_budget = m.n_over_budget;
 }
 
 } // extern "C"

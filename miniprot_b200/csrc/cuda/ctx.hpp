@@ -44,6 +44,8 @@ struct mpb_ctx_s {
 	// chaining / seeding / refinement arenas
 	mpb::cuda::DevBuf b_c[16];
 	mpb::cuda::PinBuf h_c[4];
+	// the working arenas above (every DevBuf except the resident index and the --spsc table) and their budget
+	mpb::cuda::Ledger mem;
 
 	mpb_stats_t stats;
 	mpb::Stages *stages = 0;

@@ -115,9 +115,10 @@ int nasw_check_ie_coef(float ie_coef)
 	return nsw::ext_len_penalty(ie_coef, 2147483646) == t.val[t.n - 1] ? 0 : -1;
 }
 
-// run jobs[lo, hi) as one sub-wave
+// run jobs[lo, hi) as one sub-wave; room >= 0: the bytes the ledger gives the arenas of the stage (they hold nothing live before the
+// sub-wave: those larger than it needs are released when keeping them would crowd the others out of the room)
 static void run_subwave(mpb_ctx_s *ctx, const Switches &sw, const uint8_t *packed, const uint8_t *d_ss, const char *d_aa, const NaswConst &cst, const ns_opt_t *nso,
-                        std::vector<DpDev> &jobs, size_t lo, size_t hi, DpSet &out)
+                        std::vector<DpDev> &jobs, size_t lo, size_t hi, int64_t room, DpSet &out)
 {
 	const int n = (int)(hi - lo);
 	if (n == 0) return;
@@ -209,6 +210,13 @@ static void run_subwave(mpb_ctx_s *ctx, const Switches &sw, const uint8_t *packe
 			unit_count[b][c] = (int)units.size() - unit_first[b][c];
 		}
 	n_units_tot = (int)units.size();
+	if (room >= 0)
+		ctx->mem.trim({ &ctx->b_units, &ctx->b_jobs, &ctx->b_order, &ctx->b_chunks, &ctx->b_rw, &ctx->b_out, &ctx->b_carry, &ctx->b_tb, &ctx->b_cigar, &ctx->b_cigpack,
+		                &ctx->b_cigoff },
+		              { (sizeof(int2) + sizeof(int)) * (size_t)n_units_tot + 64, sizeof(DpDev) * n, sizeof(int) * (flat.size() + 1),
+		                sizeof(PrepChunk) * (chunks.size() + pchunks.size() + 1), 32 * (size_t)(rw_tot + 4), sizeof(int4) * n, sizeof(int) * (size_t)(carry_tot + 4),
+		                sizeof(uint16_t) * (size_t)(tb_tot + 8), sizeof(uint32_t) * (size_t)(cig_tot + 4), cig_tot ? sizeof(uint32_t) * (size_t)(cig_tot + 4) : 0,
+		                cig_tot ? sizeof(int64_t) * (size_t)(n + 1) : 0 }, room);
 	if (n_units_tot) {
 		ctx->b_units.reserve((sizeof(int2) + sizeof(int)) * (size_t)n_units_tot + 64);
 		MPB_CUDA_OK(cudaMemcpyAsync(ctx->b_units.p, units.data(), sizeof(int2) * units.size(), cudaMemcpyHostToDevice, st));
@@ -378,20 +386,49 @@ void nasw_run(mpb_ctx_s *ctx, const uint8_t *packed, const uint8_t *d_ss, const 
 	out.cig.clear(), out.cig_off.assign(n + 1, 0);
 	if (n == 0) return;
 	const Switches sw = Switches::from_env();
+	const nsw::PairLimits plim = pair_limits(base);
 	NaswConst cst;
 	fill_const(base, cst);
+	Busy busy({ &ctx->b_jobs, &ctx->b_order, &ctx->b_chunks, &ctx->b_rw, &ctx->b_out, &ctx->b_carry, &ctx->b_tb, &ctx->b_cigar, &ctx->b_cigpack, &ctx->b_cigoff, &ctx->b_units });
+	ClaimScope claim(ctx->mem);
+	auto arenas_held = [&]() {
+		int64_t h = 0;
+		for (DevBuf *b : busy.v) h += (int64_t)b->cap;
+		return h;
+	};
+	// Sub-waves also stop at the ledger's room (less the quarter reserve() may add), asked for when a sub-wave does not fit what the
+	// arenas of this stage hold, and always under an explicit budget
+	int64_t lim = -1;
 	size_t lo = 0;
 	while (lo < n) {
 		size_t hi = lo, tb_bytes = 0, rw_bytes = 0;
-		while (hi < n) {
-			const DpDev &j = jobs[hi];
-			const bool is_tb = !(j.flag & (NS_F_EXT_LEFT | NS_F_EXT_RIGHT));
-			const bool v3 = use_v3(sw);
-			const int C = pick_C(j.al), Wp = v3 ? 32 * v3_warps(sw, j.al) : 32 * C, W8 = (j.al + 7) / 8 * 8, n_pass = (W8 + Wp - 1) / Wp;
-			const size_t tbb = is_tb ? (size_t)n_pass * (size_t)(j.nl + 3 * Wp + 64) * Wp * 2 : 0, rwb = (size_t)(j.nl + 20) * 32;
-			if (hi > lo && (tb_bytes + tbb > kTbBudget || rw_bytes + rwb > kRwBudget)) break;
-			tb_bytes += tbb, rw_bytes += rwb, ++hi;
+		int64_t all_bytes = 0;
+		for (int pass = 0; pass < 2; ++pass) {
+			hi = lo, tb_bytes = rw_bytes = 0, all_bytes = 0;
+			while (hi < n) {
+				const DpDev &j = jobs[hi];
+				const bool is_tb = !(j.flag & (NS_F_EXT_LEFT | NS_F_EXT_RIGHT));
+				const bool v3 = use_v3(sw);
+				const int C = pick_C(j.al), Wp = v3 ? 32 * v3_warps(sw, j.al) : 32 * C, W8 = (j.al + 7) / 8 * 8, n_pass = (W8 + Wp - 1) / Wp;
+				const size_t tbb = is_tb ? (size_t)n_pass * (size_t)(j.nl + 3 * Wp + 64) * Wp * 2 : 0, rwb = (size_t)(j.nl + 20) * 32;
+				// every arena of the problem, an upper bound: traceback and row records (as run_subwave lays them out for the pair-lane
+				// kernels), CIGAR slots and their packed copy, the carry rows of a multi-pass problem, prep chunks, descriptors
+				const bool pair = use_pair(sw, j, base, plim);
+				const int64_t tb_all = pair ? (is_tb ? (int64_t)6 * (nsw::pair_n_macro(j.nl, W8) + 2) * 64 : 0) : (int64_t)tbb;
+				const int64_t rw_all = pair ? (int64_t)192 * 32 * nsw::pair_rec_blocks(j.nl) : (int64_t)rwb;
+				const int64_t allb = tb_all + rw_all + (int64_t)8 * (j.nl + j.al + 4) + (n_pass > 1 ? (int64_t)16 * (j.nl + 3 * Wp + 64) : 0) +
+				                     (int64_t)sizeof(PrepChunk) * (j.nl / PREP_ROWS + 2) + 256 + 12 * n_pass;
+				if (hi > lo && (tb_bytes + tbb > kTbBudget || rw_bytes + rwb > kRwBudget || (lim >= 0 && all_bytes + allb > lim))) break;
+				tb_bytes += tbb, rw_bytes += rwb, all_bytes += allb, ++hi;
+			}
+			if (lim >= 0 || (ctx->mem.budget == 0 && all_bytes <= arenas_held())) break;
+			// (claimed until the stage ends: the first sub-wave's arenas, with reserve()'s quarter, within the room)
+			const int64_t first = all_bytes;
+			lim = std::max<int64_t>(ctx->mem.plan({ &ctx->b_jobs, &ctx->b_order, &ctx->b_chunks, &ctx->b_rw, &ctx->b_out, &ctx->b_carry, &ctx->b_tb, &ctx->b_cigar,
+			                                        &ctx->b_cigpack, &ctx->b_cigoff, &ctx->b_units },
+			                                      [&](int64_t room) { return std::min(first / 4 * 5, room); }) / 5 * 4, 0);
 		}
+		if (lim >= 0 && hi == lo + 1 && all_bytes > lim) ctx->mem.n_over_budget += 1;
 		// A problem over the budget runs in a sub-wave of its own (a whole-region alignment of --dbg-aflt over a long region).  It runs
 		// only when the device has the memory for its arenas (the current ones are freed before they grow; reserve() adds a quarter);
 		// otherwise it reports nt_len = -1 and the caller drops its region with a warning, instead of failing in cudaMalloc.
@@ -406,7 +443,8 @@ void nasw_run(mpb_ctx_s *ctx, const uint8_t *packed, const uint8_t *d_ss, const 
 				continue;
 			}
 		}
-		run_subwave(ctx, sw, packed, d_ss, d_aa, cst, base, jobs, lo, hi, out);
+		ctx->mem.n_subwaves += 1;
+		run_subwave(ctx, sw, packed, d_ss, d_aa, cst, base, jobs, lo, hi, lim >= 0 ? lim / 4 * 5 : -1, out);
 		if (oversize) ctx->b_tb.release(), ctx->b_rw.release(); // not kept past the budget: other contexts on the device need the memory
 		lo = hi;
 	}

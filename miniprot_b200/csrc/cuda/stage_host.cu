@@ -2,16 +2,21 @@
 // in HBM, kernel sequence, and the few small device->host hops needed to size the next buffers.
 //
 // S1 per mini-batch (map.c:155-195):
-//   sketch+occupancy kernel -> [D2H: anchors per protein] -> expand -> segmented sort -> pre-chain fill/backtrack
-//   (kept anchors re-sorted on device) -> main-chain fill/backtrack -> gather -> [D2H: chains + anchors]
+//   sketch+occupancy kernel -> [D2H: anchors per protein] -> per slice of proteins: expand -> segmented sort -> pre-chain
+//   fill/backtrack (kept anchors re-sorted on device) -> main-chain fill/backtrack -> gather -> [D2H: chains + anchors]
 // S2 per mini-batch (map.c:41-97):
-//   protein 5-mers -> sort -> window count -> [D2H: anchors per window] -> window emit -> segmented sort ->
+//   protein 5-mers -> sort -> window count -> [D2H: anchors per window] -> per slice of windows: window emit -> segmented sort ->
 //   chain fill/backtrack -> gather -> [D2H] -> host keeps the best chain of each window
+// The slices keep the arenas that grow with the anchors within the context's device-memory allowance (slices.hpp, devbuf.hpp
+// Ledger).  Every protein and window is independent of the rest of its batch, so the results are those of one pass; with room to
+// spare there is one slice, and the launch sequence is that of one pass over the batch.
+#include <algorithm>
 #include <numeric>
 #include "ctx.hpp"
 #include "stages_dev.hpp"
 #include "chain_dev.hpp"
 #include "seed_dev.hpp"
+#include "../slices.hpp"
 
 namespace mpb {
 namespace cuda {
@@ -50,6 +55,62 @@ struct Carver {
 };
 template <class F> static size_t carve_size(F f) { Carver c(0); f(c); return c.used + 256; }
 
+// chain scratch of n_prob problems over N anchors (b_c[8]): 72 B per anchor, a stack of CHAIN_STACK * 24 B and a few counters per problem
+struct ChainScratch {
+	int32_t *f, *p, *t, *v, *d_nu, *d_nb, *d_nu2, *d_nb2, *d_list;
+	uint64_t *z, *du, *db, *du2, *db2, *gu, *gb;
+	int64_t *d_go_u, *d_go_b;
+	void *stack;
+	void layout(Carver &c, int n_prob, size_t N)
+	{
+		f = c.take<int32_t>(N + 1), p = c.take<int32_t>(N + 1), t = c.take<int32_t>(N + 1), v = c.take<int32_t>(N + 1);
+		z = c.take<uint64_t>(N + 1);
+		d_list = c.take<int32_t>((size_t)n_prob);
+		du = c.take<uint64_t>(N + 1), db = c.take<uint64_t>(N + 1), du2 = c.take<uint64_t>(N + 1), db2 = c.take<uint64_t>(N + 1);
+		gu = c.take<uint64_t>(N + 1), gb = c.take<uint64_t>(N + 1);
+		d_nu = c.take<int32_t>((size_t)n_prob), d_nb = c.take<int32_t>((size_t)n_prob), d_nu2 = c.take<int32_t>((size_t)n_prob), d_nb2 = c.take<int32_t>((size_t)n_prob);
+		d_go_u = c.take<int64_t>((size_t)n_prob + 1), d_go_b = c.take<int64_t>((size_t)n_prob + 1);
+		stack = c.take<char>((size_t)n_prob * CHAIN_STACK * 24);
+	}
+	static size_t bytes(int n_prob, size_t N) { ChainScratch s; return carve_size([&](Carver &c) { s.layout(c, n_prob, N); }); }
+};
+
+// ---- slices -----------------------------------------------------------------------------------------------------------------
+// Arena bytes of a slice: per anchor the anchors and the sort's ping-pong buffer (b_c[1] / b_c[2] or b_c[5] / b_c[6], 16 B) and, when
+// it is chained, the chain scratch (b_c[8], 72 B); per problem its chain stack, counters and sort descriptors; per slice the
+// alignment of the carved pieces and the arenas' rounding.
+static const int64_t kAnchorBytesChain = 88, kAnchorBytesSeed = 16, kProbBytes = (int64_t)CHAIN_STACK * 24 + 128, kSliceFixed = (int64_t)64 << 10;
+
+static inline size_t anchor_arena(size_t N) { return sizeof(uint64_t) * (N + 2); }
+
+// Cuts the items [0, n) (cnt[i] anchors each) of a stage whose sliced arenas are `mine`: one slice, without asking the device, when
+// the budget is automatic and the whole batch fits what they hold (`whole`: each arena's need for one pass); else greedy slices
+// within the room the ledger gives them, less the quarter reserve() may add, and the largest slice (with that quarter) is claimed
+// until the stage ends (the caller holds a ClaimScope).  Returns that room, or -1 for the first case.
+static int64_t plan_items(mpb_ctx_s *ctx, std::initializer_list<DevBuf*> mine, std::initializer_list<size_t> whole, int n, const int64_t *cnt, int64_t per_anchor,
+                          SlicePlan &p, int64_t &n_slices)
+{
+	int64_t room = -1;
+	if (ctx->mem.budget == 0 && Ledger::fits(mine, whole)) {
+		p.cut.assign(1, 0), p.cut.push_back(n), p.n_over = 0;
+	} else {
+		std::vector<int64_t> bytes((size_t)n);
+		for (int i = 0; i < n; ++i) bytes[(size_t)i] = cnt[i] * per_anchor + kProbBytes;
+		room = ctx->mem.plan(mine, [&](int64_t r) {
+			plan_slices(n, bytes.data(), cnt, kSliceFixed, r / 5 * 4, kSliceMaxCount, p);
+			int64_t most = 0;
+			for (int k = 0; k < p.n_slices(); ++k) {
+				int64_t s = kSliceFixed;
+				for (int i = p.cut[(size_t)k]; i < p.cut[(size_t)k + 1]; ++i) s += bytes[(size_t)i];
+				most = std::max(most, s);
+			}
+			return most / 4 * 5;
+		});
+	}
+	n_slices += p.n_slices(), ctx->mem.n_over_budget += p.n_over;
+	return room;
+}
+
 // chain n_prob problems whose sorted anchors sit in d_a at d_off[]; returns per-problem chains and compacted anchors
 // on the host.  pre != null runs the block-level pre-chain first (map.c:186-192).
 static void chain_problems(mpb_ctx_s *ctx, int n_prob, const std::vector<int64_t> &h_off, const int64_t *d_off, uint64_t *d_a, const chn::Par *pre, const chn::Par &mainp,
@@ -59,25 +120,14 @@ static void chain_problems(mpb_ctx_s *ctx, int n_prob, const std::vector<int64_t
 	const size_t N = (size_t)h_off[(size_t)n_prob];
 	n_u.assign((size_t)n_prob, 0), n_b.assign((size_t)n_prob, 0), u.clear(), bb.clear();
 	if (n_prob == 0) return;
-	int32_t *f, *p, *t, *v, *d_nu, *d_nb, *d_nu2, *d_nb2;
-	uint64_t *z;
-	int32_t *d_list;
-	uint64_t *du, *db, *du2, *db2, *gu, *gb;
-	int64_t *d_go_u, *d_go_b;
-	void *stack;
-	auto layout = [&](Carver &c) {
-		f = c.take<int32_t>(N + 1), p = c.take<int32_t>(N + 1), t = c.take<int32_t>(N + 1), v = c.take<int32_t>(N + 1);
-		z = c.take<uint64_t>(N + 1);
-		d_list = c.take<int32_t>((size_t)n_prob);
-		du = c.take<uint64_t>(N + 1), db = c.take<uint64_t>(N + 1), du2 = c.take<uint64_t>(N + 1), db2 = c.take<uint64_t>(N + 1);
-		gu = c.take<uint64_t>(N + 1), gb = c.take<uint64_t>(N + 1);
-		d_nu = c.take<int32_t>((size_t)n_prob), d_nb = c.take<int32_t>((size_t)n_prob), d_nu2 = c.take<int32_t>((size_t)n_prob), d_nb2 = c.take<int32_t>((size_t)n_prob);
-		d_go_u = c.take<int64_t>((size_t)n_prob + 1), d_go_b = c.take<int64_t>((size_t)n_prob + 1);
-		stack = c.take<char>((size_t)n_prob * CHAIN_STACK * 24);
-	};
-	ctx->b_c[8].reserve(carve_size(layout));
+	ChainScratch cs;
+	ctx->b_c[8].reserve(ChainScratch::bytes(n_prob, N));
 	Carver cv(ctx->b_c[8].p);
-	layout(cv);
+	cs.layout(cv, n_prob, N);
+	int32_t *f = cs.f, *p = cs.p, *t = cs.t, *v = cs.v, *d_nu = cs.d_nu, *d_nb = cs.d_nb, *d_nu2 = cs.d_nu2, *d_nb2 = cs.d_nb2, *d_list = cs.d_list;
+	uint64_t *z = cs.z, *du = cs.du, *db = cs.db, *du2 = cs.du2, *db2 = cs.db2, *gu = cs.gu, *gb = cs.gb;
+	int64_t *d_go_u = cs.d_go_u, *d_go_b = cs.d_go_b;
+	void *stack = cs.stack;
 	// Size classes (from the offsets: an upper bound for a main chain that follows a pre-chain), run concurrently on side
 	// streams:  0: <= 2048 anchors   fill + backtrack fused in one warp with ALL state in shared memory (32 KB, 7 warps per SM)
 	//           1..NC-1: up to 16384 anchors in steps of ~1 K   global-memory fill (every problem its own warp, ~1000 in
@@ -160,6 +210,7 @@ void chain_batch_run(mpb_ctx_s *ctx, const chn::Par &par, int n_prob, const int6
                      std::vector<uint64_t> &u, std::vector<uint64_t> &bb)
 {
 	cudaStream_t st = ctx->stream;
+	Busy busy({ &ctx->b_c[1], &ctx->b_c[7], &ctx->b_c[8] });
 	std::vector<int64_t> off(a_off, a_off + n_prob + 1);
 	const size_t N = (size_t)off[(size_t)n_prob];
 	ctx->b_c[1].reserve(sizeof(uint64_t) * (N + 2));
@@ -170,15 +221,18 @@ void chain_batch_run(mpb_ctx_s *ctx, const chn::Par &par, int n_prob, const int6
 	chain_problems(ctx, n_prob, off, ctx->b_c[7].as<int64_t>(), ctx->b_c[1].as<uint64_t>(), 0, chn::normalise(par), n_u, n_b, u, bb);
 }
 
-// Seeding of a batch (map.c:155-177 per query): sketch, adaptive occupancy cut-off, expansion of the index buckets, sort.
-// On return a_off[n_q + 1] delimits each query's sorted anchors inside the device array *d_a_out (ctx->b_c[1]); *d_off_out is
-// the same table on the device.
-static void seed_run(mpb_ctx_s *ctx, const mp_idx_t *mi, int32_t max_occ, const Batch &b, const std::vector<int32_t> &aa_off, const char *d_aa,
-                     std::vector<int64_t> &a_off, uint64_t **d_a_out, int64_t **d_off_out)
+// Seeding of a batch (map.c:155-177 per query): sketch, adaptive occupancy cut-off [D2H: anchors per query], then per slice of
+// queries the expansion of the index buckets and the sort, handed to fn(q0, q1, a_off, d_a_off, d_a): a_off[q1 - q0 + 1] delimits
+// each query's sorted anchors (from 0) inside d_a (ctx->b_c[1]), d_a_off is the same table on the device.  chain: fn chains the
+// slice (the plan leaves room for the chain scratch).
+template <class F>
+static void seed_run(mpb_ctx_s *ctx, const mp_idx_t *mi, int32_t max_occ, const Batch &b, const std::vector<int32_t> &aa_off, const char *d_aa, bool chain, F fn)
 {
 	cudaStream_t st = ctx->stream;
 	const int n_q = b.n;
 	const size_t R = (size_t)aa_off[(size_t)n_q];
+	Busy busy({ &ctx->b_aa, &ctx->b_c[0], &ctx->b_c[1], &ctx->b_c[2], &ctx->b_c[3], &ctx->b_c[8] });
+	ClaimScope claim(ctx->mem);
 	SeedConst cst;
 	mp_mapopt_t tmp;
 	memset(&tmp, 0, sizeof(tmp));
@@ -199,48 +253,75 @@ static void seed_run(mpb_ctx_s *ctx, const mp_idx_t *mi, int32_t max_occ, const 
 	ctx->time_begin();
 	seed_launch_sketch(st, d_aa, d_aa_off, n_q, cst, ctx->d_ki, sd_hash, sd_pos, sd_cnt, sd_aoff, d_nsd, d_tot);
 	std::vector<int64_t> tot((size_t)n_q);
-	a_off.assign((size_t)n_q + 1, 0);
 	MPB_CUDA_OK(cudaMemcpyAsync(tot.data(), d_tot, sizeof(int64_t) * (size_t)n_q, cudaMemcpyDeviceToHost, st));
-	MPB_CUDA_OK(cudaStreamSynchronize(st));
-	for (int q = 0; q < n_q; ++q) a_off[(size_t)q + 1] = a_off[(size_t)q] + tot[(size_t)q];
-	const size_t N = (size_t)a_off[(size_t)n_q];
-	MPB_CUDA_OK(cudaMemcpyAsync(d_a_off, a_off.data(), sizeof(int64_t) * a_off.size(), cudaMemcpyHostToDevice, st));
-	ctx->b_c[1].reserve(sizeof(uint64_t) * (N + 2));
-	ctx->b_c[2].reserve(sizeof(uint64_t) * (N + 2));
-	uint64_t *d_a = ctx->b_c[1].as<uint64_t>(), *d_tmp = ctx->b_c[2].as<uint64_t>();
-	seed_launch_expand(st, d_aa_off, n_q, ctx->d_ki, ctx->d_kb, sd_hash, sd_pos, sd_cnt, sd_aoff, d_nsd, d_a_off, d_a);
-	seg_sort_u64(ctx, st, d_a, d_tmp, n_q, a_off.data(), a_off.data() + 1);
 	ctx->stats.ms_seed += ctx->time_end();
-	ctx->stats.kernel_launches += 3;
-	ctx->stats.n_anchors += (int64_t)N;
-	*d_a_out = d_a, *d_off_out = d_a_off;
+	ctx->stats.kernel_launches += 1;
+	const size_t N_all = (size_t)std::accumulate(tot.begin(), tot.end(), (int64_t)0);
+	SlicePlan plan;
+	const int64_t room = plan_items(ctx, { &ctx->b_c[1], &ctx->b_c[2], &ctx->b_c[8] },
+	                                { anchor_arena(N_all), anchor_arena(N_all), chain ? ChainScratch::bytes(n_q, N_all) : 0 }, n_q, tot.data(),
+	                                chain ? kAnchorBytesChain : kAnchorBytesSeed, plan, ctx->mem.n_slices_seed);
+	std::vector<int64_t> a_off;
+	for (int k = 0; k < plan.n_slices(); ++k) {
+		const int q0 = plan.cut[(size_t)k], n = plan.cut[(size_t)k + 1] - q0;
+		a_off.assign((size_t)n + 1, 0);
+		for (int q = 0; q < n; ++q) a_off[(size_t)q + 1] = a_off[(size_t)q] + tot[(size_t)(q0 + q)];
+		const size_t N = (size_t)a_off[(size_t)n];
+		if (room >= 0) ctx->mem.trim({ &ctx->b_c[1], &ctx->b_c[2], &ctx->b_c[8] }, { anchor_arena(N), anchor_arena(N), chain ? ChainScratch::bytes(n, N) : 0 }, room);
+		ctx->time_begin();
+		MPB_CUDA_OK(cudaMemcpyAsync(d_a_off, a_off.data(), sizeof(int64_t) * a_off.size(), cudaMemcpyHostToDevice, st));
+		ctx->b_c[1].reserve(anchor_arena(N));
+		ctx->b_c[2].reserve(anchor_arena(N));
+		uint64_t *d_a = ctx->b_c[1].as<uint64_t>(), *d_tmp = ctx->b_c[2].as<uint64_t>();
+		seed_launch_expand(st, d_aa_off + q0, n, ctx->d_ki, ctx->d_kb, sd_hash, sd_pos, sd_cnt, sd_aoff, d_nsd + q0, d_a_off, d_a);
+		seg_sort_u64(ctx, st, d_a, d_tmp, n, a_off.data(), a_off.data() + 1);
+		ctx->stats.ms_seed += ctx->time_end();
+		ctx->stats.kernel_launches += 2;
+		ctx->stats.n_anchors += (int64_t)N;
+		fn(q0, q0 + n, a_off, (const int64_t*)d_a_off, d_a);
+	}
+}
+
+// sorted anchors of a slice -> appended to a host array (seed_off[q0] is set; seed_off[q0 + 1 ..] are)
+static void append_anchors(mpb_ctx_s *ctx, int q0, const std::vector<int64_t> &a_off, const uint64_t *d_a, std::vector<int64_t> &off, std::vector<uint64_t> &a)
+{
+	const int n = (int)a_off.size() - 1;
+	const size_t at = a.size();
+	a.resize(at + (size_t)a_off[(size_t)n]);
+	if (a.size() > at) MPB_CUDA_OK(cudaMemcpyAsync(a.data() + at, d_a, sizeof(uint64_t) * (a.size() - at), cudaMemcpyDeviceToHost, ctx->stream));
+	MPB_CUDA_OK(cudaStreamSynchronize(ctx->stream));
+	ctx->stats.d2h_bytes += (int64_t)(sizeof(uint64_t) * (a.size() - at));
+	for (int q = 0; q < n; ++q) off[(size_t)(q0 + q) + 1] = off[(size_t)q0] + a_off[(size_t)q + 1];
 }
 
 // stage-level entry for tests/benchmarks: seeding only (mpb_seed_batch)
 void seed_batch_run(mpb_ctx_s *ctx, const mp_idx_t *mi, int32_t max_occ, const Batch &b, const std::vector<int32_t> &aa_off, const char *d_aa,
                     std::vector<int64_t> &a_off, std::vector<uint64_t> &a)
 {
-	uint64_t *d_a = 0;
-	int64_t *d_off = 0;
 	a_off.assign((size_t)b.n + 1, 0), a.clear();
 	if (b.n == 0) return;
-	seed_run(ctx, mi, max_occ, b, aa_off, d_aa, a_off, &d_a, &d_off);
-	a.resize((size_t)a_off[(size_t)b.n]);
-	if (!a.empty()) MPB_CUDA_OK(cudaMemcpyAsync(a.data(), d_a, sizeof(uint64_t) * a.size(), cudaMemcpyDeviceToHost, ctx->stream));
-	MPB_CUDA_OK(cudaStreamSynchronize(ctx->stream));
-	ctx->stats.d2h_bytes += (int64_t)(sizeof(uint64_t) * a.size());
+	seed_run(ctx, mi, max_occ, b, aa_off, d_aa, false, [&](int q0, int, const std::vector<int64_t> &so, const int64_t *, uint64_t *d_a) {
+		append_anchors(ctx, q0, so, d_a, a_off, a);
+	});
 }
 
-// map.c:186-195: pre-chain and main chain of every query's sorted seeds (d_a at a_off)
-static void chain_seeds(mpb_ctx_s *ctx, const mp_idx_t *mi, const mp_mapopt_t *opt, int n_q, const std::vector<int64_t> &a_off, const int64_t *d_a_off, uint64_t *d_a,
+// map.c:186-195: pre-chain and main chain of the sorted seeds of queries [q0, q0 + n) (d_a at a_off, from 0), appended to out
+static void chain_seeds(mpb_ctx_s *ctx, const mp_idx_t *mi, const mp_mapopt_t *opt, int q0, const std::vector<int64_t> &a_off, const int64_t *d_a_off, uint64_t *d_a,
                         ChainSet &out)
 {
+	const int n = (int)a_off.size() - 1;
 	const int32_t w = 1 << mi->opt.bbit, spl = !(opt->flag & MP_F_NO_SPLICE);
 	const chn::Par pre = chain_par(w, w, w, opt, 2, 0, mi->opt.kmer, mi->opt.bbit);
 	const chn::Par mainp = chain_par(opt->max_intron, opt->max_gap, opt->bw, opt, opt->min_chn_cnt, opt->min_chn_sc, mi->opt.kmer, mi->opt.bbit);
 	std::vector<int32_t> n_u, n_b;
-	chain_problems(ctx, n_q, a_off, d_a_off, d_a, (!(opt->flag & MP_F_NO_PRE_CHAIN) && spl) ? &pre : 0, mainp, n_u, n_b, out.u, out.a);
-	for (int q = 0; q < n_q; ++q) out.u_off[(size_t)q + 1] = out.u_off[(size_t)q] + n_u[(size_t)q], out.a_off[(size_t)q + 1] = out.a_off[(size_t)q] + n_b[(size_t)q];
+	std::vector<uint64_t> u, bb;
+	chain_problems(ctx, n, a_off, d_a_off, d_a, (!(opt->flag & MP_F_NO_PRE_CHAIN) && spl) ? &pre : 0, mainp, n_u, n_b, u, bb);
+	for (int q = 0; q < n; ++q) {
+		const size_t g = (size_t)(q0 + q);
+		out.u_off[g + 1] = out.u_off[g] + n_u[(size_t)q], out.a_off[g + 1] = out.a_off[g] + n_b[(size_t)q];
+	}
+	if (out.u.empty()) out.u.swap(u); else out.u.insert(out.u.end(), u.begin(), u.end());
+	if (out.a.empty()) out.a.swap(bb); else out.a.insert(out.a.end(), bb.begin(), bb.end());
 }
 
 void seed_chain_run(mpb_ctx_s *ctx, const mp_idx_t *mi, const mp_mapopt_t *opt, const Batch &b, const std::vector<int32_t> &aa_off, const char *d_aa, ChainSet &out)
@@ -248,32 +329,28 @@ void seed_chain_run(mpb_ctx_s *ctx, const mp_idx_t *mi, const mp_mapopt_t *opt, 
 	const int n_q = b.n;
 	out.u_off.assign((size_t)n_q + 1, 0), out.a_off.assign((size_t)n_q + 1, 0), out.u.clear(), out.a.clear();
 	if (n_q == 0) return;
-	std::vector<int64_t> a_off;
-	uint64_t *d_a = 0;
-	int64_t *d_a_off = 0;
-	seed_run(ctx, mi, opt->max_occ, b, aa_off, d_aa, a_off, &d_a, &d_a_off);
-	if (out.want_seeds) { // --dbg-anchor: the sorted seeds, before the chaining stages reuse the buffers
-		out.seed_off = a_off;
-		out.seed.resize((size_t)a_off[(size_t)n_q]);
-		if (!out.seed.empty()) MPB_CUDA_OK(cudaMemcpyAsync(out.seed.data(), d_a, sizeof(uint64_t) * out.seed.size(), cudaMemcpyDeviceToHost, ctx->stream));
-		MPB_CUDA_OK(cudaStreamSynchronize(ctx->stream));
-		ctx->stats.d2h_bytes += (int64_t)(sizeof(uint64_t) * out.seed.size());
-	}
-	chain_seeds(ctx, mi, opt, n_q, a_off, d_a_off, d_a, out);
+	if (out.want_seeds) out.seed_off.assign((size_t)n_q + 1, 0), out.seed.clear();
+	seed_run(ctx, mi, opt->max_occ, b, aa_off, d_aa, true, [&](int q0, int, const std::vector<int64_t> &a_off, const int64_t *d_a_off, uint64_t *d_a) {
+		if (out.want_seeds) append_anchors(ctx, q0, a_off, d_a, out.seed_off, out.seed); // --dbg-anchor: the sorted seeds, before chaining reuses the buffers
+		chain_seeds(ctx, mi, opt, q0, a_off, d_a_off, d_a, out);
+	});
 }
 
 // Seeding of a batch of loci (map_loci): query q against contig q of the locus view vi only, exactly what the reference seeds from an
 // index of that locus alone.  There is no k-mer table; per batch:
 //   protein seeds (prot_kmer_kernel with the mod filter) -> sort per protein -> ORF scan of both strands of every locus, keeping the
-//   k-mers whose bucket the protein has (count, [D2H], emit) -> sort + unique per locus: its (bucket, block) pairs, as index.c:71-90
-//   holds them -> bucket sizes, adaptive occupancy cut-off, anchor offsets [D2H] -> seed_expand_kernel -> sort per query.
-// On return a_off[n_q + 1] delimits each query's sorted anchors (view block ids) inside *d_a_out (ctx->b_c[1]).
-static void seed_loci_run(mpb_ctx_s *ctx, const mp_idx_t *vi, int32_t max_occ, const Batch &b, const std::vector<int32_t> &aa_off, const char *d_aa,
-                          std::vector<int64_t> &a_off, uint64_t **d_a_out, int64_t **d_off_out)
+//   k-mers whose bucket the protein has (count [D2H]); then per slice of pairs (20 B per join pair: the pairs, their distinct keys and
+//   blocks): emit -> sort + unique per locus: its (bucket, block) pairs, as index.c:71-90 holds them -> bucket sizes, adaptive
+//   occupancy cut-off, anchors per pair [D2H]; and per slice of those pairs by anchors: seed_expand_kernel -> sort per query, handed
+//   to fn as seed_run does.
+template <class F>
+static void seed_loci_run(mpb_ctx_s *ctx, const mp_idx_t *vi, int32_t max_occ, const Batch &b, const std::vector<int32_t> &aa_off, const char *d_aa, bool chain, F fn)
 {
 	cudaStream_t st = ctx->stream;
 	const int n_q = b.n;
 	const size_t R = (size_t)aa_off[(size_t)n_q];
+	Busy busy({ &ctx->b_aa, &ctx->b_c[0], &ctx->b_c[1], &ctx->b_c[2], &ctx->b_c[3], &ctx->b_c[4], &ctx->b_c[5], &ctx->b_c[6], &ctx->b_c[8] });
+	ClaimScope claim(ctx->mem);
 	SeedConst cst;
 	mp_mapopt_t tmp;
 	memset(&tmp, 0, sizeof(tmp));
@@ -324,41 +401,72 @@ static void seed_loci_run(mpb_ctx_s *ctx, const mp_idx_t *vi, int32_t max_occ, c
 		for (int q = 0; q < n_q; ++q) sb[(size_t)q] = aa_off[(size_t)q], se[(size_t)q] = aa_off[(size_t)q] + n_pk[(size_t)q];
 		seg_sort_u64(ctx, st, d_pk, d_pk_tmp, n_q, sb.data(), se.data());
 	}
-	// the join: count, then emit at per-unit offsets
+	// the join's count pass over every locus
 	locus_launch_join(st, false, d_units, n_units, d_strands, ctx->d_seq, cst, vi->opt.min_aa_len, vi->opt.bbit, d_pk, d_aa_off, d_npk, 0, d_unit_n, 0);
-	std::vector<int64_t> unit_n((size_t)n_units + 1, 0), unit_off((size_t)n_units + 1, 0), seg((size_t)n_q + 1, 0);
+	std::vector<int64_t> unit_n((size_t)n_units + 1, 0), m_q((size_t)n_q, 0);
 	if (n_units) MPB_CUDA_OK(cudaMemcpyAsync(unit_n.data(), d_unit_n, sizeof(int64_t) * (size_t)n_units, cudaMemcpyDeviceToHost, st));
-	MPB_CUDA_OK(cudaStreamSynchronize(st));
-	for (int u = 0; u < n_units; ++u) unit_off[(size_t)u + 1] = unit_off[(size_t)u] + unit_n[(size_t)u];
-	for (int q = 0; q <= n_q; ++q) seg[(size_t)q] = unit_off[unit_first[(size_t)q]];
-	const size_t M = (size_t)seg[(size_t)n_q];
-	MPB_CUDA_OK(cudaMemcpyAsync(d_unit_off, unit_off.data(), sizeof(int64_t) * unit_off.size(), cudaMemcpyHostToDevice, st));
-	MPB_CUDA_OK(cudaMemcpyAsync(d_seg, seg.data(), sizeof(int64_t) * seg.size(), cudaMemcpyHostToDevice, st));
-	ctx->b_c[4].reserve(sizeof(uint64_t) * (M + 2)), ctx->b_c[5].reserve(sizeof(uint64_t) * (M + 2)), ctx->b_c[6].reserve(sizeof(uint32_t) * (M + 2));
-	uint64_t *d_pairs = ctx->b_c[4].as<uint64_t>(), *d_uniq = ctx->b_c[5].as<uint64_t>();
-	uint32_t *d_blk = ctx->b_c[6].as<uint32_t>();
-	locus_launch_join(st, true, d_units, n_units, d_strands, ctx->d_seq, cst, vi->opt.min_aa_len, vi->opt.bbit, d_pk, d_aa_off, d_npk, d_unit_off, 0, d_pairs);
-	seg_sort_u64(ctx, st, d_pairs, d_uniq, n_q, seg.data(), seg.data() + 1);
-	locus_launch_unique(st, d_pairs, d_seg, n_q, d_uniq, d_blk, d_nu);
-	// bucket sizes, occupancy cut-off, expansion
-	locus_launch_occ(st, d_pk, d_aa_off, d_npk, n_q, d_uniq, d_seg, d_nu, max_occ, sd_idx, sd_pos, sd_lo, sd_cnt, sd_aoff, d_tot);
-	std::vector<int64_t> tot((size_t)n_q);
-	a_off.assign((size_t)n_q + 1, 0);
-	MPB_CUDA_OK(cudaMemcpyAsync(tot.data(), d_tot, sizeof(int64_t) * (size_t)n_q, cudaMemcpyDeviceToHost, st));
-	MPB_CUDA_OK(cudaStreamSynchronize(st));
-	for (int q = 0; q < n_q; ++q) a_off[(size_t)q + 1] = a_off[(size_t)q] + tot[(size_t)q];
-	const size_t N = (size_t)a_off[(size_t)n_q];
-	MPB_CUDA_OK(cudaMemcpyAsync(d_a_off, a_off.data(), sizeof(int64_t) * a_off.size(), cudaMemcpyHostToDevice, st));
-	ctx->b_c[1].reserve(sizeof(uint64_t) * (N + 2));
-	ctx->b_c[2].reserve(sizeof(uint64_t) * (N + 2));
-	uint64_t *d_a = ctx->b_c[1].as<uint64_t>(), *d_tmp = ctx->b_c[2].as<uint64_t>();
-	seed_launch_expand(st, d_aa_off, n_q, sd_lo, d_blk, sd_idx, sd_pos, sd_cnt, sd_aoff, d_npk, d_a_off, d_a);
-	seg_sort_u64(ctx, st, d_a, d_tmp, n_q, a_off.data(), a_off.data() + 1);
 	ctx->stats.ms_seed += ctx->time_end();
-	MPB_CUDA_OK(cudaGetLastError());
-	ctx->stats.kernel_launches += 6;
-	ctx->stats.n_anchors += (int64_t)N;
-	*d_a_out = d_a, *d_off_out = d_a_off;
+	ctx->stats.kernel_launches += 2;
+	for (int q = 0; q < n_q; ++q)
+		for (size_t u = unit_first[(size_t)q]; u < unit_first[(size_t)q + 1]; ++u) m_q[(size_t)q] += unit_n[u];
+	const size_t M_all = (size_t)std::accumulate(m_q.begin(), m_q.end(), (int64_t)0);
+	// slices of pairs by join pairs: a quarter of the room, the rest is for the anchors of the slices inside
+	SlicePlan outer;
+	const int64_t room_p = plan_items(ctx, { &ctx->b_c[4], &ctx->b_c[5], &ctx->b_c[6] }, { anchor_arena(M_all), anchor_arena(M_all), sizeof(uint32_t) * (M_all + 2) }, n_q,
+	                                  m_q.data(), 20 * 4, outer, ctx->mem.n_slices_loci);
+	const int64_t per_anchor = chain ? kAnchorBytesChain : kAnchorBytesSeed;
+	std::vector<int64_t> unit_off, seg, tot, a_off;
+	for (int k = 0; k < outer.n_slices(); ++k) {
+		const int p0 = outer.cut[(size_t)k], np = outer.cut[(size_t)k + 1] - p0;
+		const size_t u0 = unit_first[(size_t)p0], nu = unit_first[(size_t)(p0 + np)] - u0;
+		unit_off.assign(nu + 1, 0), seg.assign((size_t)np + 1, 0);
+		for (size_t u = 0; u < nu; ++u) unit_off[u + 1] = unit_off[u] + unit_n[u0 + u];
+		for (int q = 0; q <= np; ++q) seg[(size_t)q] = unit_off[unit_first[(size_t)(p0 + q)] - u0];
+		const size_t M = (size_t)seg[(size_t)np];
+		if (room_p >= 0) ctx->mem.trim({ &ctx->b_c[4], &ctx->b_c[5], &ctx->b_c[6] }, { anchor_arena(M), anchor_arena(M), sizeof(uint32_t) * (M + 2) }, room_p);
+		ctx->time_begin();
+		MPB_CUDA_OK(cudaMemcpyAsync(d_unit_off, unit_off.data(), sizeof(int64_t) * unit_off.size(), cudaMemcpyHostToDevice, st));
+		MPB_CUDA_OK(cudaMemcpyAsync(d_seg, seg.data(), sizeof(int64_t) * seg.size(), cudaMemcpyHostToDevice, st));
+		ctx->b_c[4].reserve(anchor_arena(M)), ctx->b_c[5].reserve(anchor_arena(M)), ctx->b_c[6].reserve(sizeof(uint32_t) * (M + 2));
+		uint64_t *d_pairs = ctx->b_c[4].as<uint64_t>(), *d_uniq = ctx->b_c[5].as<uint64_t>();
+		uint32_t *d_blk = ctx->b_c[6].as<uint32_t>();
+		locus_launch_join(st, true, d_units + u0, (int)nu, d_strands, ctx->d_seq, cst, vi->opt.min_aa_len, vi->opt.bbit, d_pk, d_aa_off, d_npk, d_unit_off, 0, d_pairs);
+		seg_sort_u64(ctx, st, d_pairs, d_uniq, np, seg.data(), seg.data() + 1);
+		locus_launch_unique(st, d_pairs, d_seg, np, d_uniq, d_blk, d_nu + p0);
+		// bucket sizes, occupancy cut-off
+		locus_launch_occ(st, d_pk, d_aa_off + p0, d_npk + p0, np, d_uniq, d_seg, d_nu + p0, max_occ, sd_idx, sd_pos, sd_lo, sd_cnt, sd_aoff, d_tot + p0);
+		tot.assign((size_t)np, 0);
+		MPB_CUDA_OK(cudaMemcpyAsync(tot.data(), d_tot + p0, sizeof(int64_t) * (size_t)np, cudaMemcpyDeviceToHost, st));
+		ctx->stats.ms_seed += ctx->time_end();
+		ctx->stats.kernel_launches += 3;
+		// expansion, by slices of anchors
+		const size_t N_all = (size_t)std::accumulate(tot.begin(), tot.end(), (int64_t)0);
+		SlicePlan inner;
+		const int64_t room = plan_items(ctx, { &ctx->b_c[1], &ctx->b_c[2], &ctx->b_c[8] },
+		                                { anchor_arena(N_all), anchor_arena(N_all), chain ? ChainScratch::bytes(np, N_all) : 0 }, np, tot.data(), per_anchor, inner,
+		                                ctx->mem.n_slices_loci);
+		ctx->mem.n_slices_loci -= 1; // an outer slice counts as its inner slices
+		for (int j = 0; j < inner.n_slices(); ++j) {
+			const int r0 = inner.cut[(size_t)j], n = inner.cut[(size_t)j + 1] - r0;
+			a_off.assign((size_t)n + 1, 0);
+			for (int q = 0; q < n; ++q) a_off[(size_t)q + 1] = a_off[(size_t)q] + tot[(size_t)(r0 + q)];
+			const size_t N = (size_t)a_off[(size_t)n];
+			if (room >= 0) ctx->mem.trim({ &ctx->b_c[1], &ctx->b_c[2], &ctx->b_c[8] }, { anchor_arena(N), anchor_arena(N), chain ? ChainScratch::bytes(n, N) : 0 }, room);
+			ctx->time_begin();
+			MPB_CUDA_OK(cudaMemcpyAsync(d_a_off, a_off.data(), sizeof(int64_t) * a_off.size(), cudaMemcpyHostToDevice, st));
+			ctx->b_c[1].reserve(anchor_arena(N));
+			ctx->b_c[2].reserve(anchor_arena(N));
+			uint64_t *d_a = ctx->b_c[1].as<uint64_t>(), *d_tmp = ctx->b_c[2].as<uint64_t>();
+			const int q0 = p0 + r0;
+			seed_launch_expand(st, d_aa_off + q0, n, sd_lo, d_blk, sd_idx, sd_pos, sd_cnt, sd_aoff, d_npk + q0, d_a_off, d_a);
+			seg_sort_u64(ctx, st, d_a, d_tmp, n, a_off.data(), a_off.data() + 1);
+			ctx->stats.ms_seed += ctx->time_end();
+			MPB_CUDA_OK(cudaGetLastError());
+			ctx->stats.kernel_launches += 1;
+			ctx->stats.n_anchors += (int64_t)N;
+			fn(q0, q0 + n, a_off, (const int64_t*)d_a_off, d_a);
+		}
+	}
 }
 
 void seed_chain_loci_run(mpb_ctx_s *ctx, const mp_idx_t *vi, const mp_mapopt_t *opt, const Batch &b, const std::vector<int32_t> &aa_off, const char *d_aa, ChainSet &out)
@@ -366,26 +474,20 @@ void seed_chain_loci_run(mpb_ctx_s *ctx, const mp_idx_t *vi, const mp_mapopt_t *
 	const int n_q = b.n;
 	out.u_off.assign((size_t)n_q + 1, 0), out.a_off.assign((size_t)n_q + 1, 0), out.u.clear(), out.a.clear();
 	if (n_q == 0) return;
-	std::vector<int64_t> a_off;
-	uint64_t *d_a = 0;
-	int64_t *d_a_off = 0;
-	seed_loci_run(ctx, vi, opt->max_occ, b, aa_off, d_aa, a_off, &d_a, &d_a_off);
-	chain_seeds(ctx, vi, opt, n_q, a_off, d_a_off, d_a, out);
+	seed_loci_run(ctx, vi, opt->max_occ, b, aa_off, d_aa, true, [&](int q0, int, const std::vector<int64_t> &a_off, const int64_t *d_a_off, uint64_t *d_a) {
+		chain_seeds(ctx, vi, opt, q0, a_off, d_a_off, d_a, out);
+	});
 }
 
 // stage-level entry for tests: locus seeding only (mpb_seed_loci_batch)
 void seed_loci_batch_run(mpb_ctx_s *ctx, const mp_idx_t *vi, int32_t max_occ, const Batch &b, const std::vector<int32_t> &aa_off, const char *d_aa,
                          std::vector<int64_t> &a_off, std::vector<uint64_t> &a)
 {
-	uint64_t *d_a = 0;
-	int64_t *d_off = 0;
 	a_off.assign((size_t)b.n + 1, 0), a.clear();
 	if (b.n == 0) return;
-	seed_loci_run(ctx, vi, max_occ, b, aa_off, d_aa, a_off, &d_a, &d_off);
-	a.resize((size_t)a_off[(size_t)b.n]);
-	if (!a.empty()) MPB_CUDA_OK(cudaMemcpyAsync(a.data(), d_a, sizeof(uint64_t) * a.size(), cudaMemcpyDeviceToHost, ctx->stream));
-	MPB_CUDA_OK(cudaStreamSynchronize(ctx->stream));
-	ctx->stats.d2h_bytes += (int64_t)(sizeof(uint64_t) * a.size());
+	seed_loci_run(ctx, vi, max_occ, b, aa_off, d_aa, false, [&](int q0, int, const std::vector<int64_t> &so, const int64_t *, uint64_t *d_a) {
+		append_anchors(ctx, q0, so, d_a, a_off, a);
+	});
 }
 
 void refine_run(mpb_ctx_s *ctx, const mp_idx_t *mi, const mp_mapopt_t *opt, const Batch &b, const std::vector<int32_t> &aa_off, const char *d_aa,
@@ -397,6 +499,8 @@ void refine_run(mpb_ctx_s *ctx, const mp_idx_t *mi, const mp_mapopt_t *opt, cons
 	out.off.assign((size_t)n_j + 1, 0), out.a.clear(), out.sc.assign((size_t)n_j, 0);
 	if (n_j == 0) return;
 	if (mi->opt.min_aa_len > WIN_MAX_MIN_AA) { fprintf(stderr, "[miniprot_b200] min ORF length %d > %d is not supported by the window kernel\n", mi->opt.min_aa_len, WIN_MAX_MIN_AA); abort(); }
+	Busy busy({ &ctx->b_aa, &ctx->b_c[3], &ctx->b_c[4], &ctx->b_c[5], &ctx->b_c[6], &ctx->b_c[8] });
+	ClaimScope claim(ctx->mem);
 	SeedConst cst;
 	fill_seed_const(mi, opt, cst);
 	const int k2 = opt->kmer2;
@@ -439,39 +543,50 @@ void refine_run(mpb_ctx_s *ctx, const mp_idx_t *mi, const mp_mapopt_t *opt, cons
 	}
 	MPB_CUDA_OK(cudaMemcpyAsync(d_wj, wj.data(), sizeof(WinJob) * (size_t)n_j, cudaMemcpyHostToDevice, st));
 	win_launch_count(st, d_wj, n_j, ctx->d_seq, cst, k2, mi->opt.min_aa_len, opt->max_ava, d_pk, d_aa_off, d_npk, d_grp, d_na);
-	std::vector<int64_t> na((size_t)n_j), a_off((size_t)n_j + 1, 0);
+	std::vector<int64_t> na((size_t)n_j), a_off;
 	MPB_CUDA_OK(cudaMemcpyAsync(na.data(), d_na, sizeof(int64_t) * (size_t)n_j, cudaMemcpyDeviceToHost, st));
-	MPB_CUDA_OK(cudaStreamSynchronize(st));
-	for (int j = 0; j < n_j; ++j) a_off[(size_t)j + 1] = a_off[(size_t)j] + na[(size_t)j];
-	const size_t N = (size_t)a_off[(size_t)n_j];
-	MPB_CUDA_OK(cudaMemcpyAsync(d_a_off, a_off.data(), sizeof(int64_t) * a_off.size(), cudaMemcpyHostToDevice, st));
-	ctx->b_c[5].reserve(sizeof(uint64_t) * (N + 2));
-	ctx->b_c[6].reserve(sizeof(uint64_t) * (N + 2));
-	uint64_t *d_a = ctx->b_c[5].as<uint64_t>(), *d_tmp = ctx->b_c[6].as<uint64_t>();
-	win_launch_emit(st, d_wj, n_j, ctx->d_seq, cst, k2, mi->opt.min_aa_len, d_pk, d_aa_off, d_npk, d_grp, d_a_off, d_a);
-	seg_sort_u64(ctx, st, d_a, d_tmp, n_j, a_off.data(), a_off.data() + 1);
 	ctx->stats.ms_refine += ctx->time_end();
-	ctx->stats.kernel_launches += 5;
+	ctx->stats.kernel_launches += 3;
 	ctx->stats.n_refine_regions += n_j;
 	const chn::Par par = chain_par(opt->max_intron, opt->max_gap, opt->bw, opt, opt->min_chn_cnt, opt->min_chn_sc, k2, 0);
+	const size_t N_all = (size_t)std::accumulate(na.begin(), na.end(), (int64_t)0);
+	SlicePlan plan;
+	const int64_t room = plan_items(ctx, { &ctx->b_c[5], &ctx->b_c[6], &ctx->b_c[8] }, { anchor_arena(N_all), anchor_arena(N_all), ChainScratch::bytes(n_j, N_all) }, n_j,
+	                                na.data(), kAnchorBytesChain, plan, ctx->mem.n_slices_refine);
 	std::vector<int32_t> n_u, n_b;
 	std::vector<uint64_t> u, bb;
-	chain_problems(ctx, n_j, a_off, d_a_off, d_a, 0, par, n_u, n_b, u, bb);
-	// keep the best-scoring chain of each window (first maximum, map.c:88-96)
-	size_t uo = 0, bo = 0;
-	for (int j = 0; j < n_j; ++j) {
-		const int32_t nu = n_u[(size_t)j];
-		if (nu > 0) {
-			int32_t best = 0, mx = (int32_t)(u[uo] >> 32);
-			for (int32_t i = 1; i < nu; ++i) if (mx < (int32_t)(u[uo + (size_t)i] >> 32)) mx = (int32_t)(u[uo + (size_t)i] >> 32), best = i;
-			size_t k = 0;
-			for (int32_t i = 0; i < best; ++i) k += (uint32_t)u[uo + (size_t)i];
-			const uint32_t cnt = (uint32_t)u[uo + (size_t)best];
-			out.a.insert(out.a.end(), bb.begin() + (ptrdiff_t)(bo + k), bb.begin() + (ptrdiff_t)(bo + k + cnt));
-			out.sc[(size_t)j] = mx;
+	for (int k = 0; k < plan.n_slices(); ++k) {
+		const int j0 = plan.cut[(size_t)k], n = plan.cut[(size_t)k + 1] - j0;
+		a_off.assign((size_t)n + 1, 0);
+		for (int j = 0; j < n; ++j) a_off[(size_t)j + 1] = a_off[(size_t)j] + na[(size_t)(j0 + j)];
+		const size_t N = (size_t)a_off[(size_t)n];
+		if (room >= 0) ctx->mem.trim({ &ctx->b_c[5], &ctx->b_c[6], &ctx->b_c[8] }, { anchor_arena(N), anchor_arena(N), ChainScratch::bytes(n, N) }, room);
+		ctx->time_begin();
+		MPB_CUDA_OK(cudaMemcpyAsync(d_a_off, a_off.data(), sizeof(int64_t) * a_off.size(), cudaMemcpyHostToDevice, st));
+		ctx->b_c[5].reserve(anchor_arena(N));
+		ctx->b_c[6].reserve(anchor_arena(N));
+		uint64_t *d_a = ctx->b_c[5].as<uint64_t>(), *d_tmp = ctx->b_c[6].as<uint64_t>();
+		win_launch_emit(st, d_wj + j0, n, ctx->d_seq, cst, k2, mi->opt.min_aa_len, d_pk, d_aa_off, d_npk, d_grp, d_a_off, d_a);
+		seg_sort_u64(ctx, st, d_a, d_tmp, n, a_off.data(), a_off.data() + 1);
+		ctx->stats.ms_refine += ctx->time_end();
+		ctx->stats.kernel_launches += 2;
+		chain_problems(ctx, n, a_off, d_a_off, d_a, 0, par, n_u, n_b, u, bb);
+		// keep the best-scoring chain of each window (first maximum, map.c:88-96)
+		size_t uo = 0, bo = 0;
+		for (int j = 0; j < n; ++j) {
+			const int32_t nu = n_u[(size_t)j];
+			if (nu > 0) {
+				int32_t best = 0, mx = (int32_t)(u[uo] >> 32);
+				for (int32_t i = 1; i < nu; ++i) if (mx < (int32_t)(u[uo + (size_t)i] >> 32)) mx = (int32_t)(u[uo + (size_t)i] >> 32), best = i;
+				size_t kk = 0;
+				for (int32_t i = 0; i < best; ++i) kk += (uint32_t)u[uo + (size_t)i];
+				const uint32_t cnt = (uint32_t)u[uo + (size_t)best];
+				out.a.insert(out.a.end(), bb.begin() + (ptrdiff_t)(bo + kk), bb.begin() + (ptrdiff_t)(bo + kk + cnt));
+				out.sc[(size_t)(j0 + j)] = mx;
+			}
+			out.off[(size_t)(j0 + j) + 1] = (int64_t)out.a.size();
+			uo += (size_t)nu, bo += (size_t)n_b[(size_t)j];
 		}
-		out.off[(size_t)j + 1] = (int64_t)out.a.size();
-		uo += (size_t)nu, bo += (size_t)n_b[(size_t)j];
 	}
 }
 
