@@ -393,7 +393,9 @@ void mpb_reset_stats(mpb_ctx_t *ctx); /* also resets the counters of mpb_get_mem
  * may hold at most `bytes` at once; 0 (the default) is automatic: what they hold plus the device's free memory less a sixteenth of the device (at least 1 GiB), asked of
  * the device only when an arena has to grow.  The seeding, refinement and DP stages run a batch in consecutive slices of proteins,
  * locus pairs, windows and DP problems whose arenas fit, and idle arenas of the other stages are released, largest first, when
- * one has to grow past the allowance.  Results do not depend on the budget.  A single item that does not fit on its own runs alone
+ * one has to grow past the allowance.  The k-mer index build of mp_idx_load (on the default context) sorts its (bucket, block)
+ * pairs in passes over ranges of buckets whose scratch fits (n_index_passes), at most 64 of them: below the 64th of its need a pass
+ * runs over the allowance (n_over_budget); the resident tables themselves are not capped.  Results do not depend on the budget.  A single item that does not fit on its own runs alone
  * anyway (n_over_budget), and may still fail to allocate.  Applies from the next call; idle arenas above a new budget are released
  * at once.  Returns 0, or -1 for a null context or a negative value.  MPB_DEVICE_MEM=<n>[k|m|g], read when a context is created,
  * sets the budget of every context, the default one included (an invalid value is reported and leaves automatic mode). */
@@ -407,6 +409,7 @@ typedef struct {
 	int64_t n_released, bytes_released; /* arenas released to make room, and their bytes */
 	int64_t n_over_budget;  /* items that ran alone above the allowance, and any other growth of an arena past it: while this is 0,
 	                         * peak_held stays within an explicit budget */
+	int64_t n_index_passes; /* passes of the k-mer index builds on the device (1 each when their scratch fits at once) */
 } mpb_mem_stats_t;
 void mpb_get_mem_stats(const mpb_ctx_t *ctx, mpb_mem_stats_t *st);
 

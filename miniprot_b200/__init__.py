@@ -130,7 +130,7 @@ class Stats(C.Structure):  # mpb_stats_t
 
 class MemStats(C.Structure):  # mpb_mem_stats_t
     _fields_ = [(f, C.c_int64) for f in ("budget", "allowance", "held", "peak_held", "n_slices_seed", "n_slices_loci", "n_slices_refine",
-                                         "n_subwaves", "n_released", "bytes_released", "n_over_budget")]
+                                         "n_subwaves", "n_released", "bytes_released", "n_over_budget", "n_index_passes")]
 
 
 class Extra(C.Structure):  # mp_extra_t without its trailing cigar[]

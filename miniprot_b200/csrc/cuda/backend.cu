@@ -625,11 +625,15 @@ static int build_index_on_device(mp_idx_t *mi)
 	forget_adopters(c);
 	if (c->own_index) forget_index(c); // the build reuses the context's own buffers
 	Busy busy(c->b_c, 16);
+	const int64_t passes0 = c->mem.n_index_passes;
 	if (idx_build_device(c, mi) != 0) return -1;
+	const long n_pass = (long)(c->mem.n_index_passes - passes0);
 	c->d_ki = c->own_ki.as<int64_t>(), c->d_kb = c->own_kb.as<uint32_t>(), c->d_seq = c->own_seq.as<uint8_t>();
 	upload_meta(c, mi);
 	c->mi = mi, c->own_index = true, c->idx_owner = 0;
-	if (mp_verbose >= 3) fprintf(stderr, "[M::%s@%.3f] built the k-mer tables on the device in %.3f s: %ld kmer-block pairs\n", __func__, mp_realtime(), mp_realtime() - t0, (long)mi->n_kb);
+	if (mp_verbose >= 3)
+		fprintf(stderr, "[M::%s@%.3f] built the k-mer tables on the device in %.3f s: %ld kmer-block pairs in %ld pass%s\n", __func__, mp_realtime(), mp_realtime() - t0,
+		        (long)mi->n_kb, n_pass, n_pass == 1 ? "" : "es");
 	return 0;
 }
 namespace { struct IdxBuildHook { IdxBuildHook() { mpb::g_idx_build_hook = build_index_on_device; } } g_idx_build_hook_init; }
@@ -1090,6 +1094,7 @@ void mpb_get_mem_stats(const mpb_ctx_t *c, mpb_mem_stats_t *st)
 	st->budget = m.budget, st->allowance = m.allowance_last, st->held = m.held, st->peak_held = m.peak;
 	st->n_slices_seed = m.n_slices_seed, st->n_slices_loci = m.n_slices_loci, st->n_slices_refine = m.n_slices_refine, st->n_subwaves = m.n_subwaves;
 	st->n_released = m.n_released, st->bytes_released = m.bytes_released, st->n_over_budget = m.n_over_budget;
+	st->n_index_passes = m.n_index_passes;
 }
 
 } // extern "C"

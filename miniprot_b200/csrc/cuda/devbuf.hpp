@@ -61,6 +61,7 @@ struct Ledger {
 	int64_t claim = 0; // bytes this context's current plan will still grow its arenas by
 	int64_t n_slices_seed = 0, n_slices_loci = 0, n_slices_refine = 0, n_subwaves = 0;
 	int64_t n_released = 0, bytes_released = 0, n_over_budget = 0;
+	int64_t n_index_passes = 0; // passes of the k-mer index builds (idx_build.cu)
 	std::vector<DevBuf*> bufs;
 
 	void add(DevBuf &b) { b.led = this, bufs.push_back(&b); }
@@ -77,7 +78,7 @@ struct Ledger {
 	// release idle arenas, largest first, until held <= target (never `keep` nor a busy one)
 	void release_idle(int64_t target, const DevBuf *keep);
 	void grow(DevBuf &b, size_t bytes);
-	void reset_counters() { n_slices_seed = n_slices_loci = n_slices_refine = n_subwaves = n_released = bytes_released = n_over_budget = 0, peak = held; }
+	void reset_counters() { n_slices_seed = n_slices_loci = n_slices_refine = n_subwaves = n_released = bytes_released = n_over_budget = n_index_passes = 0, peak = held; }
 };
 
 // a stage's claim ends with it

@@ -7,14 +7,17 @@
 //   1. idx_count_kernel   the ORF scan of win_scan.cuh over every contig strand, a CTA per range of 16 tiles: one atomic
 //                         per k-mer on the bucket counters (8 M buckets at the defaults)
 //   2. exclusive scan     bucket starts (device-wide scan below: block sums, recursion, second pass)
-//   3. idx_fill_kernel    the same scan again, (bucket << 32 | block) written at bucket start + atomic cursor
+// Steps 3-5 run once per pass over a range [lo, hi) of buckets.  The output is bucket-major, so each pass appends its piece of kb and
+// ki; with room for every pair there is one pass over [0, n_bucket) (plan_bucket_passes in slices.hpp and the ledger decide):
+//   3. idx_fill_kernel    the same scan again, (bucket << 32 | block) of the range's buckets written at bucket start - start[lo]
+//                         + atomic cursor
 //   4. bucket sort        buckets of <= 32 pairs by a warp (bitonic network over shuffles), larger ones by the segmented
-//                         sort of seg_sort.cu: the array is now globally sorted
-//   5. unique + compact   flag = differs from the left neighbour; scan of the flags; kb = low halves of the flagged keys,
-//                         ki[bucket] = scan value at the bucket's start
-// The genome is read from the 4-bit packed store in HBM (0.5 B per base and scan), the pairs are written twice (8 B) and
-// read by the sort; everything else is atomics on an 32 MB table that lives in L2.  ki / kb stay resident for mapping and are
-// copied to the host once for the ABI (mp_idx_dump, mp_idx_print_stat read them).
+//                         sort of seg_sort.cu: the pass's pairs are now sorted
+//   5. unique + compact   flag = differs from the left neighbour; scan of the flags; kb (after the earlier passes' pairs) = low
+//                         halves of the flagged keys, ki[bucket] = earlier passes' pairs + scan value at the bucket's start
+// The genome is read from the 4-bit packed store in HBM (0.5 B per base and scan, one more fill scan per extra pass), the pairs are
+// written twice (8 B) and read by the sort; everything else is atomics on an 32 MB table that lives in L2.  ki / kb stay resident for
+// mapping and are copied to the host once for the ABI (mp_idx_dump, mp_idx_print_stat read them).
 #include <algorithm>
 #include <vector>
 #include "ctx.hpp"
@@ -22,6 +25,7 @@
 #include "stages_dev.hpp"
 #include "win_scan.cuh"
 #include "../internal.hpp"
+#include "../slices.hpp"
 
 namespace mpb {
 namespace cuda {
@@ -51,15 +55,17 @@ __global__ void __launch_bounds__(SEED_THREADS) idx_count_kernel(const IdxUnit *
 	});
 }
 
+// the pairs of buckets [lo, hi), at start[b] - base (base = start[lo])
 __global__ void __launch_bounds__(SEED_THREADS) idx_fill_kernel(const IdxUnit *units, const IdxStrand *strands, const uint8_t *packed, SeedConst cst, int min_aa_len,
-                                                                int bbit, const int64_t *start, uint32_t *cur, uint64_t *keys)
+                                                                int bbit, const int64_t *start, uint32_t lo, uint32_t hi, int64_t base, uint32_t *cur, uint64_t *keys)
 {
 	extern __shared__ uint8_t sm[];
 	const uint32_t mask_mod = (1u << cst.mod_bit) - 1;
 	idx_scan_unit(units[blockIdx.x], strands, packed, cst, min_aa_len, sm, [&](uint32_t h, int64_t e, uint32_t boff) {
 		if ((h & mask_mod) != 0) return;
 		const uint32_t b = h >> cst.mod_bit;
-		keys[start[b] + atomicAdd(&cur[b], 1u)] = (uint64_t)b << 32 | (uint32_t)((e >> bbit) + boff); // sketch.c:58: block of the codon's last base
+		if (b < lo || b >= hi) return;
+		keys[start[b] - base + atomicAdd(&cur[b], 1u)] = (uint64_t)b << 32 | (uint32_t)((e >> bbit) + boff); // sketch.c:58: block of the codon's last base
 	});
 }
 
@@ -131,13 +137,13 @@ static void device_excl_scan(mpb_ctx_s *c, cudaStream_t st, Load f, int64_t n, i
 }
 
 // ---- buckets of up to 32 pairs: one warp each, bitonic network over shuffles -----------------------------------------------------
-__global__ void __launch_bounds__(256) idx_sort_small_kernel(const int64_t *start, uint32_t n_bucket, uint64_t *keys)
+__global__ void __launch_bounds__(256) idx_sort_small_kernel(const int64_t *start, uint32_t lo, uint32_t hi, int64_t base, uint64_t *keys)
 {
 	const int lane = threadIdx.x & 31;
 	const uint32_t w0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
-	for (uint32_t b = w0; b < n_bucket; b += nw) {
-		const int64_t s = start[b];
-		const int n = (int)(start[b + 1] - s);
+	for (uint32_t b = lo + w0; b < hi; b += nw) {
+		const int64_t s = start[b] - base;
+		const int n = (int)(start[b + 1] - start[b]);
 		if (n < 2 || n > 32) continue;
 		uint64_t v = lane < n ? keys[s + lane] : ~0ULL;
 		for (int k = 2; k <= 32; k <<= 1)
@@ -156,11 +162,20 @@ __global__ void __launch_bounds__(256) idx_compact_kernel(const uint64_t *keys, 
 	if (i < n && (i == 0 || keys[i] != keys[i - 1])) kb[rank[i]] = (uint32_t)keys[i];
 }
 
-__global__ void __launch_bounds__(256) idx_ki_kernel(const int64_t *start, uint32_t n_bucket, const int64_t *rank, int64_t *ki)
+// ki[lo..hi]: kb_base (the distinct pairs of the earlier passes) + rank at the bucket's start.  start[hi] - base = n, rank[n] = the
+// pass's distinct pairs, so ki[hi] is where the next pass starts, and after the last pass ki[n_bucket] = n_kb, the sentinel the
+// lookup kernels expect.
+__global__ void __launch_bounds__(256) idx_ki_kernel(const int64_t *start, uint32_t lo, uint32_t hi, int64_t base, const int64_t *rank, int64_t kb_base, int64_t *ki)
 {
-	const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
-	if (b <= n_bucket) ki[b] = rank[start[b]]; // start[n_bucket] = n, rank[n] = number of distinct pairs
+	const uint32_t b = lo + blockIdx.x * blockDim.x + threadIdx.x;
+	if (b <= hi) ki[b] = kb_base + rank[start[b] - base];
 }
+
+// Scratch of a pass: per pair the keys, the sort's ping-pong buffer and the rank (b_c[4] / b_c[5] / b_c[6], 8 B each); per pass the
+// rounding of those three arenas and of the sort's segment table (b_c[3], 4 KB each).  The segment table itself and the rank scan's
+// block sums (under 1 B per pair) grow into the fifth of the room the plan leaves.  The bucket counters and starts (b_c[2] / b_c[7],
+// 12 B per bucket) and the work units are busy arenas held before the plan: the ledger leaves them out of the room.
+static const int64_t kIdxPairBytes = 3 * 8, kIdxPassFixed = 4 * 4096;
 
 // nt (host, packed genome already read) -> ki / kb on the device of `c` and on the host; 0 on success
 int idx_build_device(mpb_ctx_s *c, mp_idx_t *mi)
@@ -202,41 +217,69 @@ int idx_build_device(mpb_ctx_s *c, mp_idx_t *mi)
 	// 1. count, 2. bucket starts
 	MPB_CUDA_OK(cudaMemsetAsync(d_cnt, 0, sizeof(uint32_t) * ((size_t)n_bucket + 1), st));
 	idx_count_kernel<<<(unsigned)units.size(), SEED_THREADS, smem, st>>>(d_units, d_str, d_seq, cst, io->min_aa_len, d_cnt);
+	c->stats.kernel_launches += 1;
 	device_excl_scan(c, st, LoadU32{ d_cnt }, (int64_t)n_bucket, d_start);
 	std::vector<uint32_t> h_cnt((size_t)n_bucket);
 	int64_t n_pairs = 0;
 	MPB_CUDA_OK(cudaMemcpyAsync(h_cnt.data(), d_cnt, sizeof(uint32_t) * (size_t)n_bucket, cudaMemcpyDeviceToHost, st));
 	MPB_CUDA_OK(cudaMemcpyAsync(&n_pairs, d_start + n_bucket, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
 	MPB_CUDA_OK(cudaStreamSynchronize(st));
-	// 3. fill
-	c->b_c[4].reserve(sizeof(uint64_t) * (size_t)(n_pairs + 2)), c->b_c[5].reserve(sizeof(uint64_t) * (size_t)(n_pairs + 2)), c->b_c[6].reserve(sizeof(int64_t) * (size_t)(n_pairs + 2));
+	// the resident tables, held before the plan so that automatic mode's allowance sees them: kb for every pair (n_kb <= n_pairs is
+	// only known after the last pass)
+	c->own_ki.reserve(sizeof(int64_t) * ((size_t)n_bucket + 1));
+	c->own_kb.reserve(sizeof(uint32_t) * (size_t)(n_pairs + 1));
+	int64_t *d_ki = c->own_ki.as<int64_t>();
+	uint32_t *d_kb = c->own_kb.as<uint32_t>();
+	// bucket ranges whose scratch fits the room the ledger gives it, less the quarter reserve() may add; the largest pass (with that
+	// quarter) is claimed until the build ends
+	ClaimScope claim(c->mem);
+	SlicePlan plan;
+	std::vector<int64_t> pass_pairs;
+	int64_t most = 0;
+	c->mem.plan({ &c->b_c[4], &c->b_c[5], &c->b_c[6] }, [&](int64_t room) {
+		plan_bucket_passes(n_bucket, h_cnt.data(), kIdxPairBytes, kIdxPassFixed, room / 5 * 4, kIdxMaxPasses, plan);
+		pass_pairs.assign((size_t)plan.n_slices(), 0), most = 0;
+		for (int k = 0; k < plan.n_slices(); ++k) {
+			for (int32_t b = plan.cut[(size_t)k]; b < plan.cut[(size_t)k + 1]; ++b) pass_pairs[(size_t)k] += h_cnt[(size_t)b];
+			most = std::max(most, pass_pairs[(size_t)k]);
+		}
+		return (kIdxPassFixed + most * kIdxPairBytes) / 4 * 5;
+	});
+	c->mem.n_index_passes += plan.n_slices(), c->mem.n_over_budget += plan.n_over;
+	c->b_c[4].reserve(sizeof(uint64_t) * (size_t)(most + 2)), c->b_c[5].reserve(sizeof(uint64_t) * (size_t)(most + 2)), c->b_c[6].reserve(sizeof(int64_t) * (size_t)(most + 2));
 	uint64_t *d_keys = c->b_c[4].as<uint64_t>(), *d_tmp = c->b_c[5].as<uint64_t>();
 	int64_t *d_rank = c->b_c[6].as<int64_t>();
-	MPB_CUDA_OK(cudaMemsetAsync(d_cnt, 0, sizeof(uint32_t) * ((size_t)n_bucket + 1), st));
-	idx_fill_kernel<<<(unsigned)units.size(), SEED_THREADS, smem, st>>>(d_units, d_str, d_seq, cst, io->min_aa_len, io->bbit, d_start, d_cnt, d_keys);
-	// 4. sort inside the buckets
 	int n_sm = 0;
 	MPB_CUDA_OK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, c->device));
-	idx_sort_small_kernel<<<n_sm * 8, 256, 0, st>>>(d_start, n_bucket, d_keys); // grid-stride over the buckets: eight CTAs per SM
-	{
-		std::vector<int64_t> sb, se;
-		int64_t acc = 0;
-		for (uint32_t b = 0; b < n_bucket; ++b) {
-			if (h_cnt[b] > 32) sb.push_back(acc), se.push_back(acc + h_cnt[b]);
-			acc += h_cnt[b];
+	int64_t base = 0, n_kb = 0; // pairs and distinct pairs of the earlier passes
+	for (int k = 0; k < plan.n_slices(); ++k) {
+		const uint32_t lo = (uint32_t)plan.cut[(size_t)k], hi = (uint32_t)plan.cut[(size_t)k + 1];
+		const int64_t n = pass_pairs[(size_t)k];
+		// 3. fill
+		MPB_CUDA_OK(cudaMemsetAsync(d_cnt + lo, 0, sizeof(uint32_t) * (size_t)(hi - lo), st));
+		if (n > 0) {
+			idx_fill_kernel<<<(unsigned)units.size(), SEED_THREADS, smem, st>>>(d_units, d_str, d_seq, cst, io->min_aa_len, io->bbit, d_start, lo, hi, base, d_cnt, d_keys);
+			// 4. sort inside the buckets
+			idx_sort_small_kernel<<<n_sm * 8, 256, 0, st>>>(d_start, lo, hi, base, d_keys); // grid-stride over the buckets: eight CTAs per SM
+			c->stats.kernel_launches += 2;
+			std::vector<int64_t> sb, se;
+			int64_t acc = 0;
+			for (uint32_t b = lo; b < hi; ++b) {
+				if (h_cnt[b] > 32) sb.push_back(acc), se.push_back(acc + h_cnt[b]);
+				acc += h_cnt[b];
+			}
+			if (!sb.empty()) seg_sort_u64(c, st, d_keys, d_tmp, (int)sb.size(), sb.data(), se.data());
 		}
-		if (!sb.empty()) seg_sort_u64(c, st, d_keys, d_tmp, (int)sb.size(), sb.data(), se.data());
+		// 5. distinct pairs -> kb, bucket starts -> ki
+		device_excl_scan(c, st, LoadFirst{ d_keys }, n, d_rank);
+		if (n > 0) idx_compact_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_keys, n, d_rank, d_kb + n_kb), c->stats.kernel_launches += 1;
+		idx_ki_kernel<<<(hi - lo + 256) / 256, 256, 0, st>>>(d_start, lo, hi, base, d_rank, n_kb, d_ki);
+		c->stats.kernel_launches += 1;
+		int64_t n_kb_pass = 0;
+		MPB_CUDA_OK(cudaMemcpyAsync(&n_kb_pass, d_rank + n, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+		MPB_CUDA_OK(cudaStreamSynchronize(st));
+		base += n, n_kb += n_kb_pass;
 	}
-	// 5. distinct pairs -> kb, bucket starts -> ki
-	device_excl_scan(c, st, LoadFirst{ d_keys }, n_pairs, d_rank);
-	int64_t n_kb = 0;
-	MPB_CUDA_OK(cudaMemcpyAsync(&n_kb, d_rank + n_pairs, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-	MPB_CUDA_OK(cudaStreamSynchronize(st));
-	c->own_ki.reserve(sizeof(int64_t) * ((size_t)n_bucket + 1));
-	c->own_kb.reserve(sizeof(uint32_t) * (size_t)(n_kb + 1));
-	if (n_pairs > 0) idx_compact_kernel<<<(unsigned)((n_pairs + 255) / 256), 256, 0, st>>>(d_keys, n_pairs, d_rank, c->own_kb.as<uint32_t>());
-	idx_ki_kernel<<<(n_bucket + 256) / 256, 256, 0, st>>>(d_start, n_bucket, d_rank, c->own_ki.as<int64_t>()); // entry n_bucket = n_kb: the sentinel the lookup kernels expect
-	c->stats.kernel_launches += 5;
 	mi->n_kb = n_kb;
 	mi->ki = (int64_t*)malloc(sizeof(int64_t) * (size_t)n_bucket);
 	mi->kb = (uint32_t*)malloc(sizeof(uint32_t) * (size_t)(n_kb ? n_kb : 1));
@@ -244,7 +287,7 @@ int idx_build_device(mpb_ctx_s *c, mp_idx_t *mi)
 	if (n_kb) MPB_CUDA_OK(cudaMemcpyAsync(mi->kb, c->own_kb.p, sizeof(uint32_t) * (size_t)n_kb, cudaMemcpyDeviceToHost, st));
 	MPB_CUDA_OK(cudaStreamSynchronize(st));
 	c->stats.h2d_bytes += (int64_t)seq_bytes, c->stats.d2h_bytes += (int64_t)(sizeof(int64_t) * n_bucket + sizeof(uint32_t) * (size_t)n_kb);
-	// the build's scratch (24 B per pair: 45 GB for a 3 Gbp genome) is not an arena of the mapping stages: give it back
+	// the build's scratch (24 B per pair in one pass: 45 GB for a 3 Gbp genome) is not an arena of the mapping stages: give it back
 	for (int k : { 2, 4, 5, 6, 7 }) c->b_c[k].release();
 	return 0;
 }
