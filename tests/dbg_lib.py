@@ -2,8 +2,8 @@
 reference's entry points: the oracle-backed host library of the CPU tests or libminiprot_b200.so.  Shared by test_host_dbg.py and
 test_gpu_dbg.py, and by tools/fuzz_cli.py for the dump lines.
 
-A child process parses the few options below as main.c does (main.c:114-201; -k -M -L -b -l only in the attached form -k5),
-loads the index, sets mp_dbg_flag and calls
+A child process parses the few options below as main.c does (main.c:114-201; -k -M -L -b -T -l only in the attached form -k5),
+builds the tables of the genetic code (-T), loads the index, sets mp_dbg_flag and calls
 mp_map_file: stdout is the PAF / GFF, stderr carries the dump lines, exactly where the reference CLI prints them."""
 import hashlib
 import json
@@ -34,7 +34,12 @@ INDEX_OPTION_SETS = [[], ["-k5"], ["-k4", "-M0"], ["-M0"], ["-M2"], ["-L6"], ["-
                      ["-b6"], ["-b7"], ["-b9"], ["-b10"], ["-l3"], ["-l4"], ["-l6"], ["-l7"], ["-l7", "-L5"], ["-l6", "-L4"],
                      ["-l7", "-L1"], ["-k5", "-M0", "-L12", "-b9", "-l4"]]
 INDEX_SWITCHES = ["--dbg-anchor", "--dbg-chain"]  # the X (seeds) and Y1 (first-round chains) lines show which stage diverged
-_IDX_FIELD = {"-k": "kmer", "-M": "mod_bit", "-L": "min_aa_len", "-b": "bbit"}
+# NCBI genetic codes (-T): every code ns_make_tables defines, and those the end-to-end runs take -- their output on tiny, tiny5 and
+# DPP3 differs from code 1's and from each other's (code 11 has code 1's tables), with the output formats below.
+TRANS_CODES = [1, 2, 3, 4, 5, 6, 9, 10, 11, 12, 13, 14, 15, 16, 21, 22, 23, 24, 25, 26, 27, 28, 29, 30, 31, 32, 33]
+TRANS_E2E_CODES = [2, 3, 6, 9, 14, 22, 23, 27, 31, 33]
+TRANS_FORMATS = [INDEX_SWITCHES, ["--gff"], ["--trans"], ["--aln"]]
+_IDX_FIELD = {"-k": "kmer", "-M": "mod_bit", "-L": "min_aa_len", "-b": "bbit", "-T": "trans_code"}
 
 
 def index_options(opts) -> tuple:
@@ -69,8 +74,13 @@ for i, a in enumerate(args):
     elif a.startswith("-j"): mo.sp_model = int(a[2:])
     elif a == "--spsc": spsc = args[i + 1]
     elif a.startswith("-K"): mo.mini_batch_size = int(a[2:])
-    elif a[:2] in ("-k", "-M", "-L", "-b"): setattr(io, {"-k": "kmer", "-M": "mod_bit", "-L": "min_aa_len", "-b": "bbit"}[a[:2]], int(a[2:]))
+    elif a == "--aln": mo.flag |= 0x80
+    elif a == "--trans": mo.flag |= 0x100
+    elif a[:2] in ("-k", "-M", "-L", "-b", "-T"): setattr(io, {"-k": "kmer", "-M": "mod_bit", "-L": "min_aa_len", "-b": "bbit", "-T": "trans_code"}[a[:2]], int(a[2:]))
     elif a[:2] == "-l": mo.kmer2 = int(a[2:])
+if L.ns_make_tables(io.trans_code) < 0:
+    sys.stderr.write(f"[ERROR] failed to find translation table {io.trans_code}\n")
+    sys.exit(101)
 L.mp_idx_load.restype = C.c_void_p
 L.mp_idx_load.argtypes = [C.c_char_p, C.c_void_p, C.c_int32]
 mi = L.mp_idx_load(files[0].encode(), C.byref(io), 4)
@@ -203,5 +213,8 @@ if __name__ == "__main__":  # --record: the reference's answers for every case o
         for name in ("DPP3", "tiny", "tiny5"):  # test_host_index_options / test_gpu_index_options
             for opts in INDEX_OPTION_SETS + [["-L41"]]:
                 ref_cli_dbg(opts + INDEX_SWITCHES, *sets[name])
+            for code in TRANS_E2E_CODES:  # test_host_trans_code / test_gpu_trans_code
+                for fmt in TRANS_FORMATS:
+                    ref_cli_dbg([f"-T{code}"] + fmt, *sets[name])
     save_record()
     print(len(_record), "answers written to", RECORD_PATH)

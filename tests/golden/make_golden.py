@@ -24,7 +24,9 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 from miniprot_b200 import synth  # noqa: E402
 
 REF = os.path.join(ROOT, "oracle", "_ref", "miniprot")
-RECORDED_TESTS = ["tests/test_oracle_pin.py", "tests/test_emu_nasw.py", "tests/test_tables.py"]
+RECORDED_TESTS = ["tests/test_oracle_pin.py", "tests/test_emu_nasw.py", "tests/test_tables.py",
+                  # the reference's tables and DP answers under every -T, and its -T<n> -d index files (test_gpu_trans_code too)
+                  "tests/test_host_trans_code.py::test_emu_trans_code", "tests/test_host_trans_code.py::test_host_index_trans_code"]
 
 
 def run(args, out):

@@ -101,6 +101,8 @@ def build_cases(d: str) -> dict:
         q0, c0 = hits[0][0], hits[0][1]
         loci += [(q0, hh[1], max(0, hh[2] - 100), hh[3] + 100) for hh in hits[1:4]] + [(q0, c0, 0, 20000), (q0, c0, ctg_len[c0] - 20000, ctg_len[c0])]
         cases[cfg] = dict(genome=gg, proteins=pp, args=[], loci=loci)
+    # the divergent set under the vertebrate mitochondrial code (-T2: AGA / AGG are stops, TGA is W, ATA is M)
+    cases["tiny5_T2"] = dict(cases["tiny5"], args=["-T2"])
     return cases
 
 

@@ -197,14 +197,48 @@ _tab_keepalive = {}
 
 def ref_tables() -> OraTab:
     """Oracle table bundle holding the REFERENCE's tables (as set up by ref_mp_start())."""
-    if "tab" not in _tab_keepalive:
-        r = reference(lambda: {f: bytes((C.c_uint8 * n).in_dll(ref(), "ref_" + sym)).hex() for f, sym, n in _TABLES}, "tables")
+    return ref_tables_for(1)
+
+
+def ref_tables_for(code: int) -> OraTab:
+    """Oracle table bundle holding the reference's tables of NCBI genetic code `code` (ref_ns_make_tables, -T); the reference is
+    left at code 1."""
+    if code not in _tab_keepalive:
+        def run():
+            r = ref()
+            assert r.ref_ns_make_tables(code) == 0, code
+            try:
+                return {f: bytes((C.c_uint8 * n).in_dll(r, "ref_" + sym)).hex() for f, sym, n in _TABLES}
+            finally:
+                r.ref_ns_make_tables(1)
+        r = reference(run, "tables", *([code] if code != 1 else []))
         arrs = {f: np.frombuffer(bytes.fromhex(r[f]), np.uint8).copy() for f, _, _ in _TABLES}
         t = OraTab()
         for f, _, _ in _TABLES:
             setattr(t, f, arrs[f].ctypes.data)
-        _tab_keepalive["tab"] = (t, arrs)
-    return _tab_keepalive["tab"][0]
+        _tab_keepalive[code] = (t, arrs)
+    return _tab_keepalive[code][0]
+
+
+def codon_array(tab: OraTab) -> np.ndarray:
+    """The 64 amino-acid codes (0..20, 20 = stop) of a table bundle's codon table, indexed by b1 << 4 | b2 << 2 | b3 (A, C, G, T = 0..3)."""
+    return np.ctypeslib.as_array((C.c_uint8 * 64).from_address(tab.codon)).copy()
+
+
+def stop_rows(nt: np.ndarray, codon: np.ndarray) -> int:
+    """Rows of a DP problem (nucleotide codes 0..4) whose codon, the three bases ending at the row, is a stop codon (20) of `codon`."""
+    nt = np.asarray(nt, np.int64)
+    a, b, d = nt[:-2], nt[1:-1], nt[2:]
+    ok = (a < 4) & (b < 4) & (d < 4)
+    return int((codon[(a << 4 | b << 2 | d)[ok]] == 20).sum())
+
+
+def codons_of(codon: np.ndarray) -> dict:
+    """{amino-acid letter: [codon as three base codes]} of a codon table (codon_array): what random_dp_problem(codons=) encodes with."""
+    out = {}
+    for c in range(64):
+        out.setdefault("ARNDCQEGHILKMFPSTWYV*X"[int(codon[c])], []).append([c >> 4, (c >> 2) & 3, c & 3])
+    return out
 
 
 def tables_from_arrays(nt4, aa20, aa13, codon, codon13):
@@ -237,7 +271,8 @@ def ref_set_stop_sc(m: np.ndarray, sc: int) -> None:
     m[:] = np.frombuffer(bytes.fromhex(reference(run, "ns_set_stop_sc", m, sc)), np.int8)
 
 
-def ref_nasw(nt: np.ndarray, aa: bytes, flag: int, mat: np.ndarray, par: dict, ss=None):
+def ref_nasw(nt: np.ndarray, aa: bytes, flag: int, mat: np.ndarray, par: dict, ss=None, code: int = 1):
+    """The reference's ns_global_gs16b under NCBI genetic code `code` (-T); the reference is left at code 1."""
     def run():
         r = ref()
         o = NsOpt()
@@ -250,14 +285,18 @@ def ref_nasw(nt: np.ndarray, aa: bytes, flag: int, mat: np.ndarray, par: dict, s
         o.sc = mat.ctypes.data
         rst = NsRst()
         ssp = ss.ctypes.data_as(C.c_void_p) if ss is not None else None
-        r.ref_ns_global_gs16b(None, nt.tobytes(), len(nt), aa, len(aa), C.byref(o), ssp, C.byref(rst))
+        assert r.ref_ns_make_tables(code) == 0, code  # o.codon points at the reference's live table
+        try:
+            r.ref_ns_global_gs16b(None, nt.tobytes(), len(nt), aa, len(aa), C.byref(o), ssp, C.byref(rst))
+        finally:
+            r.ref_ns_make_tables(1)
         cig = [rst.cigar[i] for i in range(rst.n_cigar)]
         if rst.n_cigar:
             _libc.free(rst.cigar)
         return rst.score, rst.nt_len, rst.aa_len, cig
     pars = tuple((k, par[k]) for k in ("go", "ge", "io", "fs", "xdrop", "end_bonus", "sp_null_bonus", "ie_coef")) + (tuple(par["sp"]),)
     v = reference(run, "ns_global_gs16b", np.ascontiguousarray(nt, np.uint8), aa, flag, np.ascontiguousarray(mat, np.int8), pars,
-                  b"" if ss is None else np.ascontiguousarray(ss, np.uint8), ss is None)
+                  b"" if ss is None else np.ascontiguousarray(ss, np.uint8), ss is None, *([("code", code)] if code != 1 else []))
     return v[0], v[1], v[2], v[3]
 
 
@@ -292,8 +331,10 @@ for _i, _a in enumerate(_STD):
 
 
 def random_dp_problem(rng: np.random.Generator, al_max=60, intron_max=400, p_sub=0.2, p_indel=0.03, p_fs=0.02, p_n=0.002,
-                      flank=30):
-    """A protein and a nucleotide string (codes 0..4) that encodes a mutated, intron-interrupted copy of it."""
+                      flank=30, codons=None, p_stop=0.01):
+    """A protein and a nucleotide string (codes 0..4) that encodes a mutated, intron-interrupted copy of it: with the standard
+    code, or with `codons` (codons_of() of another genetic code); a residue is replaced by a stop codon with probability p_stop."""
+    cod_of = codons or _AA2COD
     al = int(rng.integers(1, al_max + 1))
     prot = [int(x) for x in rng.integers(0, 20, size=al)]
     nt = []
@@ -303,12 +344,12 @@ def random_dp_problem(rng: np.random.Generator, al_max=60, intron_max=400, p_sub
         if r < p_indel / 2:
             continue  # residue missing from the genome (insertion in the protein)
         if r < p_indel:
-            extra = _AA2COD[_AA[int(rng.integers(0, 20))]]
+            extra = cod_of[_AA[int(rng.integers(0, 20))]]
             nt += extra[int(rng.integers(0, len(extra)))]  # extra codon (deletion)
         aa = _AA[a] if rng.random() >= p_sub else _AA[int(rng.integers(0, 20))]
-        if rng.random() < 0.01:
+        if rng.random() < p_stop:
             aa = "*"
-        cods = _AA2COD[aa]
+        cods = cod_of[aa]
         cod = list(cods[int(rng.integers(0, len(cods)))])
         if rng.random() < p_fs:
             if rng.random() < 0.5:

@@ -16,8 +16,8 @@ def hc():
     return lib
 
 
-def emu(hc, nt, aa, flag, Ccols, mat, par):
-    t = ol.ref_tables()
+def emu(hc, nt, aa, flag, Ccols, mat, par, tab=None):
+    t = tab or ol.ref_tables()
     sp = (C.c_int32 * 6)(*par["sp"])
     sc, ntl, aal = C.c_int(), C.c_int(), C.c_int()
     cig = (C.c_uint32 * (len(nt) + len(aa) + 16))()
