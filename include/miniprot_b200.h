@@ -258,6 +258,20 @@ int mpb_map_loci(mpb_ctx_t *ctx, const mp_idx_t *mi, const mp_mapopt_t *opt, int
                  const int32_t *lens, const char *const *names, int32_t n_loci, const mpb_locus_t *loci,
                  int32_t *n_reg_out, mp_reg1_t **reg_out);
 
+/* Locus sets: a protein against several candidate loci at once (the gene, its paralogs, a pseudogene, a fragment on another contig,
+ * as a translated search reports them), ranked as the reference ranks hits on a genome made of those loci alone.  Set s is
+ * loci[set_off[s] .. set_off[s+1]), all of one protein qid.  Its genome: the ranges of one contig that overlap or abut
+ * (st <= previous en) merged into their union, as separate records sorted by (cid, st) -- so the order of the loci does not matter.
+ * reg_out[s] / n_reg_out[s] receive what the reference reports for the protein on that genome (index built with mi->opt, mapping
+ * options as given, -I not applied), secondary hits included, in the reference's order, moved to the real contigs: vid = cid<<1|rev,
+ * and vs / ve / feat[].vs / ve gain the st of the hit's own range on the + strand, len(cid) - en on the - strand.  A set of one
+ * locus gives what mpb_map_loci() gives for that pair.  Free with mpb_regs_free(n_sets, ...).  What mi needs and what is uploaded:
+ * as mpb_map_loci().  Returns 0; -1 (nothing mapped) for a null context, a malformed locus, a null or decreasing set_off, an empty
+ * set or a set whose loci name different proteins; -3 (with a message, nothing mapped) for what mpb_map_loci() refuses. */
+int mpb_map_locus_sets(mpb_ctx_t *ctx, const mp_idx_t *mi, const mp_mapopt_t *opt, int32_t n_seq, const char *const *seqs,
+                       const int32_t *lens, const char *const *names, int32_t n_sets, const int64_t *set_off, const mpb_locus_t *loci,
+                       int32_t *n_reg_out, mp_reg1_t **reg_out);
+
 /* An index for locus mode only, from a FASTA or FASTA.gz file (genome, contig table and block offsets as mp_idx_load() sets them,
  * with the options io, or mp_idxopt_init()'s when io is NULL) or from a .mpi file (its head, as mpb_idx_load_meta(); io is ignored).
  * Nothing of a k-mer table is built, read or uploaded: ki == kb == NULL, n_kb == 0.  Enough for mpb_map_loci() and
@@ -284,6 +298,17 @@ int32_t mpb_map_loci_file_multi(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_i
                                 FILE *out);
 int32_t mpb_map_loci_file_multi_path(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_idx_t *mi, const char *prot_fn, const char *loci_fn,
                                      const mp_mapopt_t *opt, const char *out_path);
+/* Locus sets over files: as mpb_map_loci_file_multi*(), but a line of loci_fn may have a 5th field, a set label (further fields are
+ * ignored), and the lines of one (protein, label) -- or of one protein without a label -- form one set, as mpb_map_locus_sets() maps
+ * it.  For every set, in the order of its first line, writes what the reference CLI prints for the set's genome, moved to the real
+ * contigs as mpb_map_loci_file() moves a locus's output: by the st of the hit's own range, with --aln clipped at the end of that
+ * range, -u printing at most one line per set, --outn / --outs / --outc / -N / -p applied per set, and ids numbered over the whole
+ * file.  Same validation before writing, messages and return codes as mpb_map_loci_file_multi*(); the same bytes for any n_ctx
+ * and mini_batch_size (a set is never split across units). */
+int32_t mpb_map_locus_sets_file_multi(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_idx_t *mi, const char *prot_fn, const char *loci_fn,
+                                      const mp_mapopt_t *opt, FILE *out);
+int32_t mpb_map_locus_sets_file_multi_path(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_idx_t *mi, const char *prot_fn, const char *loci_fn,
+                                           const mp_mapopt_t *opt, const char *out_path);
 
 /* mp_map_file() with an explicit output stream and context (tests, benchmarks).  The index is made resident in the context before
  * anything is mapped: shared from another context that holds it, else uploaded from its host tables.  Returns 0; -1 for a null
@@ -344,6 +369,12 @@ int mpb_seed_batch(mpb_ctx_t *ctx, const mp_idx_t *mi, int32_t max_occ, int32_t 
  * debugging bits as mpb_map_loci(). */
 int mpb_seed_loci_batch(mpb_ctx_t *ctx, const mp_idx_t *mi, int32_t max_occ, int32_t n_seq, const char *const *seqs,
                         const int32_t *lens, int32_t n_loci, const mpb_locus_t *loci, int64_t *a_off, uint64_t **a);
+/* The seeding of mpb_map_locus_sets() alone: a_off[n_sets+1] / *a hold each set's sorted, max_occ-filtered anchors, the blocks
+ * numbered as in an index of the set's genome alone (its merged, sorted ranges as records).  Returns as mpb_map_locus_sets(), -3 also
+ * for an index mpb_map_batch() refuses. */
+int mpb_seed_locus_sets_batch(mpb_ctx_t *ctx, const mp_idx_t *mi, int32_t max_occ, int32_t n_seq, const char *const *seqs,
+                              const int32_t *lens, int32_t n_sets, const int64_t *set_off, const mpb_locus_t *loci, int64_t *a_off,
+                              uint64_t **a);
 
 /* Second-round refinement over a batch of windows (replaces map.c:41-97 per region): window k is [as, ae) on strand
  * vid = contig<<1|rev of query qid.  On return a_off[n_win+1] / *a hold the best chain of each window

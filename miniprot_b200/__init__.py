@@ -226,6 +226,11 @@ def lib() -> C.CDLL:
         L.mpb_map_loci_file_multi.argtypes = [C.POINTER(C.c_void_p), C.c_int32, C.POINTER(Idx), C.c_char_p, C.c_char_p, C.POINTER(MapOpt), C.c_void_p]
         L.mpb_map_loci_file_multi_path.restype = C.c_int32
         L.mpb_map_loci_file_multi_path.argtypes = [C.POINTER(C.c_void_p), C.c_int32, C.POINTER(Idx), C.c_char_p, C.c_char_p, C.POINTER(MapOpt), C.c_char_p]
+        L.mpb_map_locus_sets_file_multi.restype = C.c_int32
+        L.mpb_map_locus_sets_file_multi.argtypes = [C.POINTER(C.c_void_p), C.c_int32, C.POINTER(Idx), C.c_char_p, C.c_char_p, C.POINTER(MapOpt), C.c_void_p]
+        L.mpb_map_locus_sets_file_multi_path.restype = C.c_int32
+        L.mpb_map_locus_sets_file_multi_path.argtypes = [C.POINTER(C.c_void_p), C.c_int32, C.POINTER(Idx), C.c_char_p, C.c_char_p, C.POINTER(MapOpt),
+                                                         C.c_char_p]
         L.mpb_idx_share.argtypes = [C.c_void_p, C.c_void_p]
         L.mpb_event_begin.argtypes = [C.c_void_p]
         L.mpb_event_end_ms.restype = C.c_double
@@ -298,6 +303,10 @@ class Context:
         lib().mpb_get_mem_stats(self.h, C.byref(s))
         return s
 
+    def map_locus_sets(self, mi, mo: "MapOpt", seqs, names, sets):
+        """map_locus_sets on this context: (rc, n_reg, reg) per set of `sets` (lists of (qid, cid, st, en))."""
+        return map_locus_sets(self, mi, mo, seqs, names, sets)
+
 
 def idxopt() -> IdxOpt:
     o = IdxOpt()
@@ -363,9 +372,10 @@ def idx_load_genome(path: str, io: IdxOpt | None = None):
     return mi
 
 
-def map_loci_file(ctxs, mi, prot_path: str, loci_path: str, out_path: str = "-", mo: MapOpt | None = None) -> None:
+def map_loci_file(ctxs, mi, prot_path: str, loci_path: str, out_path: str = "-", mo: MapOpt | None = None, sets: bool = False) -> None:
     """mpb_map_loci_file_multi: proteins (FASTA) against the loci of a TSV (`protein contig start end`) on one Context or a list of
-    distinct ones, in the output format of `mo`; out_path "-" is this process's standard output."""
+    distinct ones, in the output format of `mo`; out_path "-" is this process's standard output.  sets: mpb_map_locus_sets_file_multi,
+    the lines of one (protein, 5th-column label) forming one set (map_locus_sets_file)."""
     mo = mo or mapopt()
     ctxs = [ctxs] if isinstance(ctxs, Context) else list(ctxs)
     arr = (C.c_void_p * len(ctxs))(*[c.h for c in ctxs])
@@ -378,12 +388,21 @@ def map_loci_file(ctxs, mi, prot_path: str, loci_path: str, out_path: str = "-",
         libc.fdopen.restype, libc.fdopen.argtypes = C.c_void_p, [C.c_int, C.c_char_p]
         libc.fclose.argtypes = [C.c_void_p]
         fp = libc.fdopen(os.dup(sys.stdout.fileno()), b"wb")
-        rc = L.mpb_map_loci_file_multi(arr, len(ctxs), mi, prot_path.encode(), loci_path.encode(), C.byref(mo), fp)
+        f = L.mpb_map_locus_sets_file_multi if sets else L.mpb_map_loci_file_multi
+        rc = f(arr, len(ctxs), mi, prot_path.encode(), loci_path.encode(), C.byref(mo), fp)
         libc.fclose(fp)
     else:
-        rc = L.mpb_map_loci_file_multi_path(arr, len(ctxs), mi, prot_path.encode(), loci_path.encode(), C.byref(mo), out_path.encode())
+        f = L.mpb_map_locus_sets_file_multi_path if sets else L.mpb_map_loci_file_multi_path
+        rc = f(arr, len(ctxs), mi, prot_path.encode(), loci_path.encode(), C.byref(mo), out_path.encode())
     if rc != 0:
-        raise RuntimeError(f"mpb_map_loci_file failed ({rc})")
+        raise RuntimeError(f"{'mpb_map_locus_sets_file' if sets else 'mpb_map_loci_file'} failed ({rc})")
+
+
+def map_locus_sets_file(ctxs, mi, prot_path: str, loci_path: str, out_path: str = "-", mo: MapOpt | None = None) -> None:
+    """mpb_map_locus_sets_file_multi: as map_loci_file, but the lines of the TSV of one protein and one set label (an optional 5th
+    column; no label: all lines of the protein) form one set, aligned as the reference aligns the protein against a genome of the
+    set's ranges alone."""
+    map_loci_file(ctxs, mi, prot_path, loci_path, out_path, mo, sets=True)
 
 
 def nsopt(mat=None, **over) -> NsOpt:
@@ -488,6 +507,35 @@ def map_loci(ctx: Context, mi, mo: MapOpt, seqs, names, loci, L: C.CDLL | None =
     return rc, n_reg[:nl], reg
 
 
+def _set_args(sets):
+    import numpy as np
+
+    off = np.array([0] + [len(x) for x in sets], np.int64).cumsum()
+    flat = [l for x in sets for l in x]
+    return off, len(flat), (Locus * max(len(flat), 1))(*[Locus(*l) for l in flat])
+
+
+def map_locus_sets(ctx: Context, mi, mo: MapOpt, seqs, names, sets, L: C.CDLL | None = None, fn: str = "mpb_map_locus_sets"):
+    """mpb_map_locus_sets: sets = list of lists of (qid, cid, st, en), the loci of one set naming one protein.  Returns (rc, n_reg
+    int32 array, reg array of mp_reg1_t pointers), one entry per set; free the regions with free_loci_regs.  `L` / `fn`: another
+    library exporting the same call without its context argument (the CPU tests' oracle-backed hc_map_locus_sets), ctx is then None."""
+    import numpy as np
+
+    n, _, arr, nam, lens, _ = _loci_args(seqs, [], names)
+    off, _, loc = _set_args(sets)
+    ns = len(sets)
+    n_reg = np.zeros(max(ns, 1), np.int32)
+    reg = (C.c_void_p * max(ns, 1))()
+    f = getattr(L or lib(), fn)
+    f.restype = C.c_int
+    f.argtypes = ([C.c_void_p] if ctx is not None else []) + [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
+                                                              C.c_void_p, C.c_void_p, C.c_void_p]
+    args = [C.cast(mi, C.c_void_p), C.cast(C.pointer(mo), C.c_void_p), n, C.cast(arr, C.c_void_p), lens.ctypes.data, C.cast(nam, C.c_void_p), ns,
+            off.ctypes.data, C.cast(loc, C.c_void_p), n_reg.ctypes.data, C.cast(reg, C.c_void_p)]
+    rc = f(*([ctx.h] if ctx is not None else []), *args)
+    return rc, n_reg[:ns], reg
+
+
 def free_loci_regs(n_reg, reg) -> None:
     """What mpb_regs_free does, with the C library's free (the regions of either library are libc-allocated)."""
     import ctypes.util
@@ -550,6 +598,29 @@ def seed_loci_batch(ctx: Context, mi, max_occ: int, seqs, loci):
     a = np.ctypeslib.as_array(C.cast(ap, C.POINTER(C.c_uint64)), shape=(max(int(off[nl]), 1),)).copy()[:int(off[nl])]
     L.mpb_free(ap)
     return [a[off[k]:off[k + 1]] for k in range(nl)]
+
+
+def seed_locus_sets_batch(ctx: Context, mi, max_occ: int, seqs, sets):
+    """mpb_seed_locus_sets_batch: the sorted, max_occ-filtered anchors (block<<32 | qpos, blocks of an index of the set's merged,
+    sorted ranges alone) of every set (a list of (qid, cid, st, en))."""
+    import numpy as np
+
+    n, _, arr, _, lens, _ = _loci_args(seqs, [])
+    so, _, loc = _set_args(sets)
+    ns = len(sets)
+    off = np.zeros(ns + 1, np.int64)
+    ap = C.c_void_p()
+    L = lib()
+    L.mpb_seed_locus_sets_batch.restype = C.c_int
+    L.mpb_seed_locus_sets_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.POINTER(C.c_void_p)]
+    rc = L.mpb_seed_locus_sets_batch(ctx.h, C.cast(mi, C.c_void_p), max_occ, n, C.cast(arr, C.c_void_p), lens.ctypes.data, ns, so.ctypes.data,
+                                     C.cast(loc, C.c_void_p), off.ctypes.data, C.byref(ap))
+    if rc != 0:
+        raise RuntimeError(f"mpb_seed_locus_sets_batch failed ({rc})")
+    a = np.ctypeslib.as_array(C.cast(ap, C.POINTER(C.c_uint64)), shape=(max(int(off[ns]), 1),)).copy()[:int(off[ns])]
+    L.mpb_free(ap)
+    return [a[off[k]:off[k + 1]] for k in range(ns)]
 
 
 class Window(C.Structure):  # mpb_window_t

@@ -159,10 +159,17 @@ struct CudaStages : Stages {
 	}
 	void seed_chain_loci(const mp_idx_t *vi, const mp_mapopt_t *opt, const Batch &b, ChainSet &out) override
 	{
+		std::vector<int32_t> ctg_off((size_t)b.n + 1);
+		for (int32_t q = 0; q <= b.n; ++q) ctg_off[(size_t)q] = q;
+		seed_chain_locus_sets(vi, ctg_off.data(), opt, b, out);
+	}
+	bool locus_sets() override { return true; }
+	void seed_chain_locus_sets(const mp_idx_t *vi, const int32_t *ctg_off, const mp_mapopt_t *opt, const Batch &b, ChainSet &out) override
+	{
 		need_index(vi);
 		std::vector<int32_t> off;
 		const char *d_aa = upload_residues(b, off);
-		seed_chain_loci_run(ctx, vi, opt, b, off, d_aa, out);
+		seed_chain_loci_run(ctx, vi, ctg_off, opt, b, off, d_aa, out);
 	}
 	void refine(const mp_idx_t *mi, const mp_mapopt_t *opt, const Batch &b, const std::vector<RefineJob> &jobs, RefineSet &out) override
 	{
@@ -757,38 +764,72 @@ int mpb_map_loci(mpb_ctx_t *c, const mp_idx_t *mi, const mp_mapopt_t *opt, int32
 	return map_loci(c->stages, mi, opt, n_seq, seqs, lens, names, n_loci, loci, n_reg_out, reg_out);
 }
 
+int mpb_map_locus_sets(mpb_ctx_t *c, const mp_idx_t *mi, const mp_mapopt_t *opt, int32_t n_seq, const char *const *seqs, const int32_t *lens,
+                       const char *const *names, int32_t n_sets, const int64_t *set_off, const mpb_locus_t *loci, int32_t *n_reg_out, mp_reg1_t **reg_out)
+{
+	if (!c || !opt) return -1;
+	LocusSets ls;
+	const int rc = locus_sets_make(mi, n_seq, n_sets, set_off, loci, ls);
+	if (rc != 0) return rc;
+	if (bad_scoring(opt->go, opt->ie_coef) || bad_index(mi)) return -3;
+	std::lock_guard<std::mutex> cl(c->mu);
+	MPB_CUDA_OK(cudaSetDevice(c->device));
+	return map_sets(c->stages, mi, opt, seqs, lens, names, ls, 0, n_sets, n_reg_out, reg_out);
+}
+
+// the seeding stage over canonical sets: anchors of each set with the block ids of an index of its ranges alone
+static int seed_sets(mpb_ctx_t *c, const mp_idx_t *mi, int32_t max_occ, const int32_t *lens, const char *const *seqs, const LocusSets &ls, int64_t *a_off,
+                     uint64_t **a)
+{
+	if (bad_index(mi)) return -3;
+	std::lock_guard<std::mutex> cl(c->mu);
+	MPB_CUDA_OK(cudaSetDevice(c->device));
+	const int32_t n = ls.n();
+	LocusView v(mi, (int32_t)ls.rng.size(), ls.rng.data());
+	std::vector<int32_t> ctg_off((size_t)n + 1);
+	std::vector<const char*> sp((size_t)n);
+	std::vector<int32_t> lp((size_t)n);
+	for (int32_t s = 0; s <= n; ++s) ctg_off[(size_t)s] = (int32_t)ls.off[(size_t)s];
+	for (int32_t s = 0; s < n; ++s) sp[(size_t)s] = seqs[ls.rng[(size_t)ls.off[(size_t)s]].qid], lp[(size_t)s] = lens[ls.rng[(size_t)ls.off[(size_t)s]].qid];
+	Batch b;
+	b.n = n, b.seq = sp.data(), b.len = lp.data(), b.name = 0;
+	std::vector<int64_t> ao((size_t)n + 1, 0);
+	std::vector<uint64_t> av;
+	if (n > 0) {
+		CudaStages *cs = static_cast<CudaStages*>(c->stages);
+		cs->loci_view(mi, &v.idx);
+		cs->need_index(&v.idx);
+		std::vector<int32_t> off;
+		const char *d_aa = cs->upload_residues(b, off);
+		seed_loci_batch_run(c, &v.idx, ctg_off.data(), max_occ, b, off, d_aa, ao, av);
+		cs->loci_view(0, 0);
+	}
+	for (int32_t s = 0; s <= n; ++s) a_off[s] = ao[(size_t)s];
+	for (int32_t s = 0; s < n; ++s) // view block ids -> those of an index of the set's ranges alone
+		for (int64_t j = ao[(size_t)s]; j < ao[(size_t)s + 1]; ++j) av[(size_t)j] -= (uint64_t)v.bo[(size_t)ctg_off[(size_t)s] * 2] << 32;
+	*a = (uint64_t*)malloc(sizeof(uint64_t) * (av.size() + 1));
+	if (!av.empty()) memcpy(*a, av.data(), sizeof(uint64_t) * av.size());
+	return 0;
+}
+
 int mpb_seed_loci_batch(mpb_ctx_t *c, const mp_idx_t *mi, int32_t max_occ, int32_t n_seq, const char *const *seqs, const int32_t *lens, int32_t n_loci,
                         const mpb_locus_t *loci, int64_t *a_off, uint64_t **a)
 {
 	if (!c) return -1;
 	const int rc = check_loci(mi, n_seq, n_loci, loci);
 	if (rc != 0) return rc;
-	if (bad_index(mi)) return -3;
-	std::lock_guard<std::mutex> cl(c->mu);
-	MPB_CUDA_OK(cudaSetDevice(c->device));
-	LocusView v(mi, n_loci, loci);
-	std::vector<const char*> sp((size_t)n_loci);
-	std::vector<int32_t> lp((size_t)n_loci);
-	for (int32_t k = 0; k < n_loci; ++k) sp[(size_t)k] = seqs[loci[k].qid], lp[(size_t)k] = lens[loci[k].qid];
-	Batch b;
-	b.n = n_loci, b.seq = sp.data(), b.len = lp.data(), b.name = 0;
-	std::vector<int64_t> ao((size_t)n_loci + 1, 0);
-	std::vector<uint64_t> av;
-	if (n_loci > 0) {
-		CudaStages *cs = static_cast<CudaStages*>(c->stages);
-		cs->loci_view(mi, &v.idx);
-		cs->need_index(&v.idx);
-		std::vector<int32_t> off;
-		const char *d_aa = cs->upload_residues(b, off);
-		seed_loci_batch_run(c, &v.idx, max_occ, b, off, d_aa, ao, av);
-		cs->loci_view(0, 0);
-	}
-	for (int32_t k = 0; k <= n_loci; ++k) a_off[k] = ao[(size_t)k];
-	for (int32_t k = 0; k < n_loci; ++k) // view block ids -> those of an index of the locus alone
-		for (int64_t j = ao[(size_t)k]; j < ao[(size_t)k + 1]; ++j) av[(size_t)j] -= (uint64_t)v.bo[(size_t)k * 2] << 32;
-	*a = (uint64_t*)malloc(sizeof(uint64_t) * (av.size() + 1));
-	if (!av.empty()) memcpy(*a, av.data(), sizeof(uint64_t) * av.size());
-	return 0;
+	LocusSets ls;
+	for (int32_t k = 0; k < n_loci; ++k) ls.add(loci + k, 1);
+	return seed_sets(c, mi, max_occ, lens, seqs, ls, a_off, a);
+}
+
+int mpb_seed_locus_sets_batch(mpb_ctx_t *c, const mp_idx_t *mi, int32_t max_occ, int32_t n_seq, const char *const *seqs, const int32_t *lens, int32_t n_sets,
+                              const int64_t *set_off, const mpb_locus_t *loci, int64_t *a_off, uint64_t **a)
+{
+	if (!c) return -1;
+	LocusSets ls;
+	const int rc = locus_sets_make(mi, n_seq, n_sets, set_off, loci, ls);
+	return rc != 0 ? rc : seed_sets(c, mi, max_occ, lens, seqs, ls, a_off, a);
 }
 
 int32_t mpb_map_file(mpb_ctx_t *c, const mp_idx_t *mi, const char *fn, const mp_mapopt_t *opt, FILE *out)
@@ -819,14 +860,15 @@ int32_t mpb_map_file_multi_path(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_i
 	return rc;
 }
 
-// the locus file driver on n_ctx contexts, into `out` or, when that is null, into a file created at out_path once the input is valid
+// the locus file driver (by_set: the locus set file driver) on n_ctx contexts, into `out` or, when that is null, into a file created at
+// out_path once the input is valid
 static int32_t map_loci_file_on(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_idx_t *mi, const char *prot_fn, const char *loci_fn, const mp_mapopt_t *opt,
-                                FILE *out, const char *out_path)
+                                FILE *out, const char *out_path, bool by_set = false)
 {
 	FileCtx fc;
 	if (!fc.distinct(ctx, n_ctx) || !opt || !mi) return -1;
 	LociFile in;
-	int32_t rc = loci_file_read(mi, prot_fn, loci_fn, in);
+	int32_t rc = loci_file_read(mi, prot_fn, loci_fn, in, by_set);
 	if (rc != 0) return rc;
 	if (bad_scoring(opt->go, opt->ie_coef) || bad_index(mi)) return -3;
 	FILE *fp = out ? out : fopen(out_path, "wb");
@@ -856,6 +898,18 @@ int32_t mpb_map_loci_file_multi_path(mpb_ctx_t *const *ctx, int32_t n_ctx, const
                                      const char *out_path)
 {
 	return out_path ? map_loci_file_on(ctx, n_ctx, mi, prot_fn, loci_fn, opt, 0, out_path) : -1;
+}
+
+int32_t mpb_map_locus_sets_file_multi(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_idx_t *mi, const char *prot_fn, const char *loci_fn, const mp_mapopt_t *opt,
+                                      FILE *out)
+{
+	return out ? map_loci_file_on(ctx, n_ctx, mi, prot_fn, loci_fn, opt, out, 0, true) : -1;
+}
+
+int32_t mpb_map_locus_sets_file_multi_path(mpb_ctx_t *const *ctx, int32_t n_ctx, const mp_idx_t *mi, const char *prot_fn, const char *loci_fn,
+                                           const mp_mapopt_t *opt, const char *out_path)
+{
+	return out_path ? map_loci_file_on(ctx, n_ctx, mi, prot_fn, loci_fn, opt, 0, out_path, true) : -1;
 }
 
 mp_reg1_t *mp_map(const mp_idx_t *mi, int qlen, const char *seq, int *n_reg, mp_tbuf_t *, const mp_mapopt_t *opt, const char *qname)

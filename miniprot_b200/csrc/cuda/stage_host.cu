@@ -336,15 +336,17 @@ void seed_chain_run(mpb_ctx_s *ctx, const mp_idx_t *mi, const mp_mapopt_t *opt, 
 	});
 }
 
-// Seeding of a batch of loci (map_loci): query q against contig q of the locus view vi only, exactly what the reference seeds from an
-// index of that locus alone.  There is no k-mer table; per batch:
-//   protein seeds (prot_kmer_kernel with the mod filter) -> sort per protein -> ORF scan of both strands of every locus, keeping the
+// Seeding of a batch of locus sets (map_sets): query q against contigs [ctg_off[q], ctg_off[q+1]) of the locus view vi only, exactly
+// what the reference seeds from an index of a genome made of those ranges alone.  The units of all of a query's strands are contiguous,
+// so that one segment of join pairs holds the (bucket, block) pairs of the query's whole index.  There is no k-mer table; per batch:
+//   protein seeds (prot_kmer_kernel with the mod filter) -> sort per protein -> ORF scan of both strands of every range, keeping the
 //   k-mers whose bucket the protein has (count [D2H]); then per slice of pairs (20 B per join pair: the pairs, their distinct keys and
 //   blocks): emit -> sort + unique per locus: its (bucket, block) pairs, as index.c:71-90 holds them -> bucket sizes, adaptive
 //   occupancy cut-off, anchors per pair [D2H]; and per slice of those pairs by anchors: seed_expand_kernel -> sort per query, handed
 //   to fn as seed_run does.
 template <class F>
-static void seed_loci_run(mpb_ctx_s *ctx, const mp_idx_t *vi, int32_t max_occ, const Batch &b, const std::vector<int32_t> &aa_off, const char *d_aa, bool chain, F fn)
+static void seed_loci_run(mpb_ctx_s *ctx, const mp_idx_t *vi, const int32_t *ctg_off, int32_t max_occ, const Batch &b, const std::vector<int32_t> &aa_off,
+                          const char *d_aa, bool chain, F fn)
 {
 	cudaStream_t st = ctx->stream;
 	const int n_q = b.n;
@@ -356,16 +358,18 @@ static void seed_loci_run(mpb_ctx_s *ctx, const mp_idx_t *vi, int32_t max_occ, c
 	memset(&tmp, 0, sizeof(tmp));
 	tmp.max_occ = max_occ;
 	fill_seed_const(vi, &tmp, cst);
-	std::vector<LocusStrand> strands((size_t)n_q * 2);
+	std::vector<LocusStrand> strands((size_t)ctg_off[n_q] * 2);
 	std::vector<LocusUnit> units;
 	std::vector<size_t> unit_first((size_t)n_q + 1, 0);
 	for (int q = 0; q < n_q; ++q) {
-		const mp_ctg_t *c = &vi->nt->ctg[q];
-		for (int s = 0; s < 2; ++s) {
-			LocusStrand &ls = strands[(size_t)q * 2 + s];
-			ls.g_start = s ? c->off + c->len - 1 : c->off, ls.dir = s ? -1 : 1, ls.comp = s, ls.len = c->len, ls.boff = vi->bo[q * 2 + s], ls.qid = q;
-			const int64_t step = (int64_t)WIN_TILE * 16;
-			for (int64_t p = 0; p < c->len; p += step) units.push_back(LocusUnit{ q * 2 + s, 0, p, std::min(p + step, (int64_t)c->len) });
+		for (int k = ctg_off[q]; k < ctg_off[q + 1]; ++k) {
+			const mp_ctg_t *c = &vi->nt->ctg[k];
+			for (int s = 0; s < 2; ++s) {
+				LocusStrand &ls = strands[(size_t)k * 2 + s];
+				ls.g_start = s ? c->off + c->len - 1 : c->off, ls.dir = s ? -1 : 1, ls.comp = s, ls.len = c->len, ls.boff = vi->bo[k * 2 + s], ls.qid = q;
+				const int64_t step = (int64_t)WIN_TILE * 16;
+				for (int64_t p = 0; p < c->len; p += step) units.push_back(LocusUnit{ k * 2 + s, 0, p, std::min(p + step, (int64_t)c->len) });
+			}
 		}
 		unit_first[(size_t)q + 1] = units.size();
 	}
@@ -469,23 +473,24 @@ static void seed_loci_run(mpb_ctx_s *ctx, const mp_idx_t *vi, int32_t max_occ, c
 	}
 }
 
-void seed_chain_loci_run(mpb_ctx_s *ctx, const mp_idx_t *vi, const mp_mapopt_t *opt, const Batch &b, const std::vector<int32_t> &aa_off, const char *d_aa, ChainSet &out)
+void seed_chain_loci_run(mpb_ctx_s *ctx, const mp_idx_t *vi, const int32_t *ctg_off, const mp_mapopt_t *opt, const Batch &b, const std::vector<int32_t> &aa_off,
+                         const char *d_aa, ChainSet &out)
 {
 	const int n_q = b.n;
 	out.u_off.assign((size_t)n_q + 1, 0), out.a_off.assign((size_t)n_q + 1, 0), out.u.clear(), out.a.clear();
 	if (n_q == 0) return;
-	seed_loci_run(ctx, vi, opt->max_occ, b, aa_off, d_aa, true, [&](int q0, int, const std::vector<int64_t> &a_off, const int64_t *d_a_off, uint64_t *d_a) {
+	seed_loci_run(ctx, vi, ctg_off, opt->max_occ, b, aa_off, d_aa, true, [&](int q0, int, const std::vector<int64_t> &a_off, const int64_t *d_a_off, uint64_t *d_a) {
 		chain_seeds(ctx, vi, opt, q0, a_off, d_a_off, d_a, out);
 	});
 }
 
-// stage-level entry for tests: locus seeding only (mpb_seed_loci_batch)
-void seed_loci_batch_run(mpb_ctx_s *ctx, const mp_idx_t *vi, int32_t max_occ, const Batch &b, const std::vector<int32_t> &aa_off, const char *d_aa,
-                         std::vector<int64_t> &a_off, std::vector<uint64_t> &a)
+// stage-level entry for tests: locus seeding only (mpb_seed_loci_batch, mpb_seed_locus_sets_batch)
+void seed_loci_batch_run(mpb_ctx_s *ctx, const mp_idx_t *vi, const int32_t *ctg_off, int32_t max_occ, const Batch &b, const std::vector<int32_t> &aa_off,
+                         const char *d_aa, std::vector<int64_t> &a_off, std::vector<uint64_t> &a)
 {
 	a_off.assign((size_t)b.n + 1, 0), a.clear();
 	if (b.n == 0) return;
-	seed_loci_run(ctx, vi, max_occ, b, aa_off, d_aa, false, [&](int q0, int, const std::vector<int64_t> &so, const int64_t *, uint64_t *d_a) {
+	seed_loci_run(ctx, vi, ctg_off, max_occ, b, aa_off, d_aa, false, [&](int q0, int, const std::vector<int64_t> &so, const int64_t *, uint64_t *d_a) {
 		append_anchors(ctx, q0, so, d_a, a_off, a);
 	});
 }

@@ -13,11 +13,12 @@ void seed_chain_run(mpb_ctx_s *ctx, const mp_idx_t *mi, const mp_mapopt_t *opt, 
 void refine_run(mpb_ctx_s *ctx, const mp_idx_t *mi, const mp_mapopt_t *opt, const Batch &b, const std::vector<int32_t> &aa_off, const char *d_aa,
                 const std::vector<RefineJob> &jobs, RefineSet &out);
 
-// S1 of locus mode (map_loci): query q seeded against contig q of the locus view vi alone, without a k-mer table; then the same chains
-void seed_chain_loci_run(mpb_ctx_s *ctx, const mp_idx_t *vi, const mp_mapopt_t *opt, const Batch &b, const std::vector<int32_t> &aa_off, const char *d_aa,
-                         ChainSet &out);
-void seed_loci_batch_run(mpb_ctx_s *ctx, const mp_idx_t *vi, int32_t max_occ, const Batch &b, const std::vector<int32_t> &aa_off, const char *d_aa,
-                         std::vector<int64_t> &a_off, std::vector<uint64_t> &a);
+// S1 of locus mode (map_sets): query q seeded against contigs [ctg_off[q], ctg_off[q+1]) of the locus view vi together -- its set's
+// ranges; one contig per query for a pair -- without a k-mer table; then the same chains
+void seed_chain_loci_run(mpb_ctx_s *ctx, const mp_idx_t *vi, const int32_t *ctg_off, const mp_mapopt_t *opt, const Batch &b, const std::vector<int32_t> &aa_off,
+                         const char *d_aa, ChainSet &out);
+void seed_loci_batch_run(mpb_ctx_s *ctx, const mp_idx_t *vi, const int32_t *ctg_off, int32_t max_occ, const Batch &b, const std::vector<int32_t> &aa_off,
+                         const char *d_aa, std::vector<int64_t> &a_off, std::vector<uint64_t> &a);
 
 void seed_batch_run(mpb_ctx_s *ctx, const mp_idx_t *mi, int32_t max_occ, const Batch &b, const std::vector<int32_t> &aa_off, const char *d_aa,
                     std::vector<int64_t> &a_off, std::vector<uint64_t> &a);

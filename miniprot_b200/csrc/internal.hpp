@@ -119,45 +119,77 @@ struct Stages {
 	// S1 of locus mode: query q is seeded against contig q of `view` alone, as the reference seeds from an index of that locus
 	// (index.c:52-136 over a one-record FASTA), then chained as in seed_chain
 	virtual void seed_chain_loci(const mp_idx_t * /*view*/, const mp_mapopt_t * /*opt*/, const Batch & /*b*/, ChainSet & /*out*/) {}
+	// Locus sets (map_sets).  True: seed_chain_locus_sets seeds a query against several contigs of `view` together.
+	virtual bool locus_sets() { return false; }
+	// S1 of a batch of locus sets: query q is seeded against contigs [ctg_off[q], ctg_off[q+1]) of `view` together, as the reference
+	// seeds from an index of a genome made of those contigs alone, then chained as in seed_chain.  Called for queries of several
+	// contigs only when locus_sets() is true; the default serves queries of one contig each (ctg_off[q] == q) with seed_chain_loci.
+	virtual void seed_chain_locus_sets(const mp_idx_t *view, const int32_t * /*ctg_off*/, const mp_mapopt_t *opt, const Batch &b, ChainSet &out)
+	{
+		seed_chain_loci(view, opt, b, out);
+	}
 };
 
 // ---------------------------------------------------------------- locus mode (pipeline.cpp)
-// The index of one batch of loci: contig q is the locus of pair q, a view into mi's packed genome (nothing is copied), with block ids
-// numbered over these contigs as index.c:11-26 numbers a genome's; ki / kb stay null.  Contig names are the real contigs'.
+// The index of one batch of loci: contig k is the range [st, en) of contig cid of rng[k], a view into mi's packed genome (nothing is
+// copied), with block ids numbered over these contigs as index.c:11-26 numbers a genome's; ki / kb stay null.  Contig names are the
+// real contigs'.  rng[k].qid is not read.
 struct LocusView {
 	mp_idx_t idx;
 	mp_ntdb_t nt;
 	std::vector<mp_ctg_t> ctg;
 	std::vector<uint32_t> bo;
-	LocusView(const mp_idx_t *mi, int32_t n, const mpb_locus_t *loci);
+	LocusView(const mp_idx_t *mi, int32_t n, const mpb_locus_t *rng);
 	LocusView(const LocusView &) = delete;
 	LocusView &operator=(const LocusView &) = delete;
 };
 // -1 for a malformed locus (qid or cid out of range, st < 0, en > contig length, st >= en); -3 with a message for what locus mode
 // refuses (--spsc scores, any mp_dbg_flag bit but MP_DBG_NO_KALLOC); else 0
 int check_loci(const mp_idx_t *mi, int32_t n_seq, int32_t n_loci, const mpb_locus_t *loci);
-// mpb_map_loci on a backend: pairs in batches of up to opt->mini_batch_size residues, each through map_batch over its LocusView with
-// the locus seeding stage; the regions come back in the coordinates of mi's contigs.  Returns check_loci()'s code, or -3 for a backend
-// without locus mode; nothing is mapped then.
+// Locus sets in canonical form: set s is protein rng[off[s]].qid against the genome made of the ranges rng[off[s], off[s+1]) --
+// sorted by (cid, st), ranges of one contig that overlap or abut merged into their union.  A pair of locus mode is a set of one range.
+struct LocusSets {
+	std::vector<int64_t> off{0};
+	std::vector<mpb_locus_t> rng;
+	int32_t n() const { return (int32_t)off.size() - 1; }
+	int64_t n_rng(int32_t s) const { return off[(size_t)s + 1] - off[(size_t)s]; }
+	void add(const mpb_locus_t *loci, int64_t n); // one set of n loci of one protein, any order
+};
+// The canonical sets of set s = loci[set_off[s], set_off[s+1]): -1 for a malformed locus, a null or decreasing set_off, an empty set
+// or a set whose loci name different proteins; check_loci()'s -3 refusals; else 0 with `out` filled.
+int locus_sets_make(const mp_idx_t *mi, int32_t n_seq, int32_t n_sets, const int64_t *set_off, const mpb_locus_t *loci, LocusSets &out);
+// Sets [s_lo, s_hi) of ls on a backend, the protein of a set being seqs/lens/names[qid]: batches of whole sets, up to
+// opt->mini_batch_size residues and fewer than 2^31 blocks, each through map_batch over the LocusView of its sets' ranges with the
+// set seeding stage; n_reg_out / reg_out[s - s_lo] receive set s's regions in the coordinates of mi's contigs.  -3 (nothing mapped)
+// for a backend without locus mode, or one without set seeding when a set has several ranges; else 0.
+int map_sets(Stages *st, const mp_idx_t *mi, const mp_mapopt_t *opt, const char *const *seqs, const int32_t *lens, const char *const *names, const LocusSets &ls,
+             int32_t s_lo, int32_t s_hi, int32_t *n_reg_out, mp_reg1_t **reg_out);
+// mpb_map_locus_sets on a backend: locus_sets_make()'s code, or map_sets over all the sets.
+int map_locus_sets(Stages *st, const mp_idx_t *mi, const mp_mapopt_t *opt, int32_t n_seq, const char *const *seqs, const int32_t *lens, const char *const *names,
+                   int32_t n_sets, const int64_t *set_off, const mpb_locus_t *loci, int32_t *n_reg_out, mp_reg1_t **reg_out);
+// mpb_map_loci on a backend: check_loci()'s code, or every pair mapped as a set of one locus (map_sets).
 int map_loci(Stages *st, const mp_idx_t *mi, const mp_mapopt_t *opt, int32_t n_seq, const char *const *seqs, const int32_t *lens, const char *const *names,
              int32_t n_loci, const mpb_locus_t *loci, int32_t *n_reg_out, mp_reg1_t **reg_out);
-// The inputs of the locus file driver, read whole: proteins (a repeated name stands for its last record) and the pairs of the loci
-// file in its order.
+// The inputs of the locus file drivers, read whole: proteins (a repeated name stands for its last record), the pairs of the loci file
+// in its order, and the sets the driver maps -- one per pair, or with `by_set` one per (protein, label) in the order of their first line.
 struct LociFile {
 	std::vector<std::string> names, seqs;
 	std::vector<const char*> sp, np;
 	std::vector<int32_t> len;
 	std::vector<mpb_locus_t> loci;
+	LocusSets sets;
+	bool by_set = false;
 	std::unordered_map<std::string, int32_t> qid;
 	void add_protein(const std::string &name, const std::string &seq);
 };
 // Reads prot_fn (FASTA, gzip or plain) and loci_fn (`protein contig start end` per line, 0-based, end exclusive; blank and '#' lines
-// skipped).  -1 with "file:line: why" on stderr for an unreadable file, a malformed line, an unknown protein or contig, or a bad
-// range; then check_loci()'s -3 refusals; else 0.
-int loci_file_read(const mp_idx_t *mi, const char *prot_fn, const char *loci_fn, LociFile &in);
-// mpb_map_loci_file_multi on n backends (the file driver's pipeline, with map_loci as the mapper): for every pair, in file order, the
-// output of the reference given that locus alone as the genome, in contig coordinates; ids numbered over the whole output.  Returns
-// 0, -1 for n < 1, or -3 (nothing written) for a backend without locus mode.
+// skipped; further fields ignored, except that with by_set a 5th field is the line's set label: the lines of one protein and one label,
+// or of one protein and no label, form one set).  -1 with "file:line: why" on stderr for an unreadable file, a malformed line, an
+// unknown protein or contig, or a bad range; then check_loci()'s -3 refusals; else 0.
+int loci_file_read(const mp_idx_t *mi, const char *prot_fn, const char *loci_fn, LociFile &in, bool by_set = false);
+// mpb_map_loci_file_multi / mpb_map_locus_sets_file_multi on n backends (the file driver's pipeline, with map_sets as the mapper): for
+// every set of `in`, in order, the output of the reference given the set's ranges alone as the genome, in contig coordinates; ids
+// numbered over the whole output.  Returns 0, -1 for n < 1, or -3 (nothing written) for a backend without locus mode or set seeding.
 int32_t map_loci_file(Stages *const *st, int n, const mp_idx_t *mi, const LociFile &in, const mp_mapopt_t *opt, FILE *out);
 
 // ---------------------------------------------------------------- host pipeline (pipeline.cpp, hits.cpp, align.cpp)

@@ -276,13 +276,26 @@ void map_batch(Stages *st, const mp_idx_t *mi, const mp_mapopt_t *opt, const Bat
 	lap(5);
 }
 
+// The end, on the strand of hit r of set s (in contig coordinates), of the set's range that holds the hit: en on +, len(cid) - st on -.
+// The ranges of a set are disjoint and sorted, and a hit lies in one of them: the last one that starts at or before the hit's start.
+static int64_t range_end(const mp_idx_t *mi, const LocusSets &ls, int32_t s, const mp_reg1_t *r)
+{
+	const int32_t cid = (int32_t)(r->vid >> 1), rev = r->vid & 1;
+	const int64_t clen = mi->nt->ctg[cid].len, pos = rev ? clen - r->vs - 1 : r->vs; // a base of the hit on the + strand
+	const mpb_locus_t *b = ls.rng.data() + ls.off[(size_t)s], *e = ls.rng.data() + ls.off[(size_t)s + 1];
+	const mpb_locus_t *l = std::upper_bound(b, e, std::make_pair(cid, pos), [](const std::pair<int32_t, int64_t> &x, const mpb_locus_t &y) {
+		return x.first < y.cid || (x.first == y.cid && x.second < y.st);
+	}) - 1;
+	return rev ? clen - l->st : l->en;
+}
+
 // map.c:293-326: per protein, hits in rank order subject to --outn / --outs / --outc; unmapped line with -u.  Every printed hit
 // gets the next number of a counter that runs over the whole file (the MP%06d ids of GFF / GTF, map.c:306): the hits each
 // protein will print are counted first, so that formatting -- independent per protein -- can run on the worker pool, each range
-// into its own buffer, written in order.  loci (locus mode): query q is the protein of locus loci[q], whose hits are in contig
-// coordinates but must not read the genome past the locus end (format_output's nt_lim), as the reference given the locus alone.
+// into its own buffer, written in order.  sets (locus mode): query q is the protein of set s0 + q, whose hits are in contig
+// coordinates but must not read the genome past the end of their range (format_output's nt_lim), as the reference given the set alone.
 static void write_batch(FILE *out, const mp_idx_t *mi, const mp_mapopt_t *opt, const Batch &b, const int32_t *n_reg, mp_reg1_t *const *reg, int64_t *id_counter,
-                        const mpb_locus_t *loci = 0)
+                        const LocusSets *sets = 0, int32_t s0 = 0)
 {
 	auto printed = [&](int32_t q, int32_t j, int32_t best) {
 		const mp_reg1_t *r = &reg[q][j];
@@ -308,8 +321,7 @@ static void write_batch(FILE *out, const mp_idx_t *mi, const mp_mapopt_t *opt, c
 			for (int32_t j = 0; j < n_reg[q] && j < opt->out_n; ++j) {
 				if (!printed(q, j, best)) continue;
 				++n_out;
-				int64_t nt_lim = -1; // locus end on the hit's strand: en on +, len(cid) - st on -
-				if (loci) nt_lim = (reg[q][j].vid & 1) ? mi->nt->ctg[loci[q].cid].len - loci[q].st : loci[q].en;
+				const int64_t nt_lim = sets ? range_end(mi, *sets, s0 + q, &reg[q][j]) : -1;
 				format_output(buf, mi, opt, b.name[q], b.len[q], b.seq[q], &reg[q][j], id0[(size_t)q] + n_out, j + 1, nt_lim);
 			}
 			if (n_out == 0) format_output(buf, mi, opt, b.name[q], b.len[q], b.seq[q], 0, 0, 0);
@@ -328,7 +340,8 @@ struct Unit {
 	std::vector<std::string> names, seqs; // the records (FASTA input only; the pointers below point into them)
 	std::vector<const char*> sp, np;      // the Batch view
 	std::vector<int32_t> len;
-	const mpb_locus_t *loci = 0;          // locus mode: query q is the protein of pair loci[q]
+	const LocusSets *sets = 0;            // locus mode: query q is the protein of set s0 + q
+	int32_t s0 = 0;
 	std::vector<int32_t> n_reg;
 	std::vector<mp_reg1_t*> reg;
 	int rc = 0;
@@ -382,7 +395,7 @@ int32_t run_units(Stages *const *st, int n, const mp_idx_t *mi, const mp_mapopt_
 	auto write_step = [&](int64_t i, Unit &u) {
 		if (u.rc != 0 && rc == 0) rc = u.rc;
 		const double t0 = mp_realtime();
-		write_batch(out, mi, opt, u.view(), u.n_reg.data(), u.reg.data(), &id_counter, u.loci);
+		write_batch(out, mi, opt, u.view(), u.n_reg.data(), u.reg.data(), &id_counter, u.sets, u.s0);
 		const double t1 = mp_realtime();
 		mpb_regs_free((int32_t)u.reg.size(), u.n_reg.data(), u.reg.data());
 		if (trace)
@@ -479,19 +492,19 @@ int32_t map_file_multi(Stages *const *st, int n, const mp_idx_t *mi, const char 
 
 // ---------------------------------------------------------------- locus mode
 
-LocusView::LocusView(const mp_idx_t *mi, int32_t n, const mpb_locus_t *loci) : ctg((size_t)n), bo((size_t)n * 2 + 1)
+LocusView::LocusView(const mp_idx_t *mi, int32_t n, const mpb_locus_t *rng) : ctg((size_t)n), bo((size_t)n * 2 + 1)
 {
 	memset(&idx, 0, sizeof(idx));
 	memset(&nt, 0, sizeof(nt));
 	const int32_t bbit = mi->opt.bbit;
 	int64_t acc = 0;
-	for (int32_t q = 0; q < n; ++q) {
-		const mp_ctg_t *c = &mi->nt->ctg[loci[q].cid];
-		mp_ctg_t &v = ctg[(size_t)q];
-		v.off = c->off + loci[q].st, v.len = loci[q].en - loci[q].st, v.name = c->name;
+	for (int32_t k = 0; k < n; ++k) {
+		const mp_ctg_t *c = &mi->nt->ctg[rng[k].cid];
+		mp_ctg_t &v = ctg[(size_t)k];
+		v.off = c->off + rng[k].st, v.len = rng[k].en - rng[k].st, v.name = c->name;
 		const int64_t nb = (v.len + (1 << bbit) - 1) >> bbit; // index.c:11-26
-		bo[(size_t)q * 2] = (uint32_t)acc, acc += nb;
-		bo[(size_t)q * 2 + 1] = (uint32_t)acc, acc += nb;
+		bo[(size_t)k * 2] = (uint32_t)acc, acc += nb;
+		bo[(size_t)k * 2 + 1] = (uint32_t)acc, acc += nb;
 	}
 	bo[(size_t)n * 2] = (uint32_t)acc;
 	nt.n_ctg = nt.m_ctg = n, nt.l_seq = nt.m_seq = mi->nt->l_seq, nt.seq = mi->nt->seq, nt.ctg = ctg.data();
@@ -516,13 +529,44 @@ int check_loci(const mp_idx_t *mi, int32_t n_seq, int32_t n_loci, const mpb_locu
 	return 0;
 }
 
+void LocusSets::add(const mpb_locus_t *loci, int64_t n)
+{
+	const size_t first = rng.size();
+	rng.insert(rng.end(), loci, loci + n);
+	std::sort(rng.begin() + (ptrdiff_t)first, rng.end(), [](const mpb_locus_t &x, const mpb_locus_t &y) { return x.cid < y.cid || (x.cid == y.cid && x.st < y.st); });
+	size_t k = first;
+	for (size_t i = first; i < rng.size(); ++i) {
+		if (k > first && rng[k - 1].cid == rng[i].cid && rng[i].st <= rng[k - 1].en) rng[k - 1].en = std::max(rng[k - 1].en, rng[i].en); // overlap or abut
+		else rng[k++] = rng[i];
+	}
+	rng.resize(k);
+	off.push_back((int64_t)k);
+}
+
+int locus_sets_make(const mp_idx_t *mi, int32_t n_seq, int32_t n_sets, const int64_t *set_off, const mpb_locus_t *loci, LocusSets &out)
+{
+	if (n_sets < 0 || (n_sets > 0 && (!set_off || set_off[0] != 0 || !loci))) return -1;
+	for (int32_t s = 0; s < n_sets; ++s)
+		if (set_off[s + 1] <= set_off[s] || set_off[s + 1] > INT32_MAX) return -1; // an empty set, or more loci than one call takes
+	for (int32_t s = 0; s < n_sets; ++s)
+		for (int64_t k = set_off[s] + 1; k < set_off[s + 1]; ++k)
+			if (loci[k].qid != loci[set_off[s]].qid) return -1;
+	const int rc = check_loci(mi, n_seq, n_sets > 0 ? (int32_t)set_off[n_sets] : 0, loci);
+	if (rc != 0) return rc;
+	out = LocusSets();
+	for (int32_t s = 0; s < n_sets; ++s) out.add(loci + set_off[s], set_off[s + 1] - set_off[s]);
+	return 0;
+}
+
 namespace {
 
-// map_batch's stages in locus mode: S1 is the backend's locus seeding, everything else passes through
+// map_batch's stages in locus mode: S1 is the backend's set seeding over the query -> view-contig ranges ctg_off, everything else
+// passes through
 struct LociStages : Stages {
 	Stages *in;
+	const int32_t *ctg_off = 0;
 	explicit LociStages(Stages *s) : in(s) {}
-	void seed_chain(const mp_idx_t *mi, const mp_mapopt_t *opt, const Batch &b, ChainSet &out) override { in->seed_chain_loci(mi, opt, b, out); }
+	void seed_chain(const mp_idx_t *mi, const mp_mapopt_t *opt, const Batch &b, ChainSet &out) override { in->seed_chain_locus_sets(mi, ctg_off, opt, b, out); }
 	void refine(const mp_idx_t *mi, const mp_mapopt_t *opt, const Batch &b, const std::vector<RefineJob> &jobs, RefineSet &out) override { in->refine(mi, opt, b, jobs, out); }
 	void nasw(const mp_idx_t *mi, const ns_opt_t *base, const Batch &b, const std::vector<DpJob> &jobs, DpSet &out) override { in->nasw(mi, base, b, jobs, out); }
 	void batch_begin(const Batch &b) override { in->batch_begin(b); }
@@ -531,31 +575,46 @@ struct LociStages : Stages {
 	void thread_init() override { in->thread_init(); }
 };
 
+// -3 with a message when a set of [s_lo, s_hi) has several ranges and the backend cannot seed a query against several contigs
+int check_set_seeding(Stages *st, const LocusSets &ls, int32_t s_lo, int32_t s_hi)
+{
+	for (int32_t s = s_lo; s < s_hi; ++s)
+		if (ls.n_rng(s) > 1 && !st->locus_sets()) {
+			fprintf(stderr, "[miniprot_b200] this backend cannot seed a protein against several loci at once\n");
+			return -3;
+		}
+	return 0;
+}
+
 } // namespace
 
-int map_loci(Stages *st, const mp_idx_t *mi, const mp_mapopt_t *opt, int32_t n_seq, const char *const *seqs, const int32_t *lens, const char *const *names,
-             int32_t n_loci, const mpb_locus_t *loci, int32_t *n_reg_out, mp_reg1_t **reg_out)
+int map_sets(Stages *st, const mp_idx_t *mi, const mp_mapopt_t *opt, const char *const *seqs, const int32_t *lens, const char *const *names, const LocusSets &ls,
+             int32_t s_lo, int32_t s_hi, int32_t *n_reg_out, mp_reg1_t **reg_out)
 {
-	const int rc = check_loci(mi, n_seq, n_loci, loci);
-	if (rc != 0) return rc;
-	for (int32_t k = 0; k < n_loci; ++k) n_reg_out[k] = 0, reg_out[k] = 0;
-	if (n_loci == 0) return 0;
-	LociStages ls(st);
-	for (int32_t i0 = 0; i0 < n_loci;) {
-		// a batch holds pairs until it has mini_batch_size residues (bseq.c:53-74), and fewer than 2^31 blocks
+	for (int32_t s = s_lo; s < s_hi; ++s) n_reg_out[s - s_lo] = 0, reg_out[s - s_lo] = 0;
+	if (s_lo >= s_hi) return 0;
+	if (check_set_seeding(st, ls, s_lo, s_hi) != 0) return -3;
+	LociStages lst(st);
+	for (int32_t i0 = s_lo; i0 < s_hi;) {
+		// a batch holds whole sets until it has mini_batch_size residues (bseq.c:53-74), and fewer than 2^31 blocks
 		int32_t i1 = i0;
 		int64_t residues = 0, blocks = 0;
-		while (i1 < n_loci && residues < opt->mini_batch_size) {
-			const int64_t nb = 2 * ((loci[i1].en - loci[i1].st + (1 << mi->opt.bbit) - 1) >> mi->opt.bbit);
+		while (i1 < s_hi && residues < opt->mini_batch_size) {
+			int64_t nb = 0;
+			for (int64_t k = ls.off[(size_t)i1]; k < ls.off[(size_t)i1 + 1]; ++k) nb += 2 * ((ls.rng[(size_t)k].en - ls.rng[(size_t)k].st + (1 << mi->opt.bbit) - 1) >> mi->opt.bbit);
 			if (i1 > i0 && blocks + nb >= (int64_t)1 << 31) break;
-			residues += lens[loci[i1].qid], blocks += nb, ++i1;
+			residues += lens[ls.rng[(size_t)ls.off[(size_t)i1]].qid], blocks += nb, ++i1;
 		}
 		const int32_t n = i1 - i0;
-		LocusView v(mi, n, loci + i0);
+		const int64_t r0 = ls.off[(size_t)i0];
+		const mpb_locus_t *rng = ls.rng.data() + r0; // contig k of the view is range rng[k]
+		LocusView v(mi, (int32_t)(ls.off[(size_t)i1] - r0), rng);
+		std::vector<int32_t> ctg_off((size_t)n + 1);
 		std::vector<const char*> sp((size_t)n), np((size_t)n);
 		std::vector<int32_t> lp((size_t)n);
+		for (int32_t q = 0; q <= n; ++q) ctg_off[(size_t)q] = (int32_t)(ls.off[(size_t)(i0 + q)] - r0);
 		for (int32_t q = 0; q < n; ++q) {
-			const int32_t p = loci[i0 + q].qid;
+			const int32_t p = rng[ctg_off[(size_t)q]].qid;
 			sp[(size_t)q] = seqs[p], lp[(size_t)q] = lens[p], np[(size_t)q] = names ? names[p] : 0;
 		}
 		Batch b;
@@ -564,23 +623,42 @@ int map_loci(Stages *st, const mp_idx_t *mi, const mp_mapopt_t *opt, int32_t n_s
 			fprintf(stderr, "[miniprot_b200] this backend has no locus seeding stage\n");
 			return -3;
 		}
-		map_batch(&ls, &v.idx, opt, b, n_reg_out + i0, reg_out + i0);
+		lst.ctg_off = ctg_off.data();
+		int32_t *nr = n_reg_out + (i0 - s_lo);
+		mp_reg1_t **rr = reg_out + (i0 - s_lo);
+		map_batch(&lst, &v.idx, opt, b, nr, rr);
 		st->loci_view(0, 0);
-		// locus strand -> contig strand: + adds st, - adds len(cid) - en
-		for (int32_t q = 0; q < n; ++q) {
-			const mpb_locus_t &l = loci[i0 + q];
-			const int64_t clen = mi->nt->ctg[l.cid].len;
-			for (int32_t j = 0; j < n_reg_out[i0 + q]; ++j) {
-				mp_reg1_t *r = &reg_out[i0 + q][j];
+		// view strand -> contig strand: + adds st, - adds len(cid) - en of the range the region lies on
+		for (int32_t q = 0; q < n; ++q)
+			for (int32_t j = 0; j < nr[q]; ++j) {
+				mp_reg1_t *r = &rr[q][j];
+				const mpb_locus_t &l = rng[r->vid >> 1];
 				const uint32_t rev = r->vid & 1;
-				const int64_t sh = rev ? clen - l.en : l.st;
+				const int64_t sh = rev ? mi->nt->ctg[l.cid].len - l.en : l.st;
 				r->vid = (uint32_t)l.cid << 1 | rev, r->vs += sh, r->ve += sh;
 				for (int32_t f = 0; f < r->n_feat; ++f) r->feat[f].vs += sh, r->feat[f].ve += sh;
 			}
-		}
 		i0 = i1;
 	}
 	return 0;
+}
+
+int map_locus_sets(Stages *st, const mp_idx_t *mi, const mp_mapopt_t *opt, int32_t n_seq, const char *const *seqs, const int32_t *lens, const char *const *names,
+                   int32_t n_sets, const int64_t *set_off, const mpb_locus_t *loci, int32_t *n_reg_out, mp_reg1_t **reg_out)
+{
+	LocusSets ls;
+	const int rc = locus_sets_make(mi, n_seq, n_sets, set_off, loci, ls);
+	return rc != 0 ? rc : map_sets(st, mi, opt, seqs, lens, names, ls, 0, n_sets, n_reg_out, reg_out);
+}
+
+int map_loci(Stages *st, const mp_idx_t *mi, const mp_mapopt_t *opt, int32_t n_seq, const char *const *seqs, const int32_t *lens, const char *const *names,
+             int32_t n_loci, const mpb_locus_t *loci, int32_t *n_reg_out, mp_reg1_t **reg_out)
+{
+	const int rc = check_loci(mi, n_seq, n_loci, loci);
+	if (rc != 0) return rc;
+	LocusSets ls;
+	for (int32_t k = 0; k < n_loci; ++k) ls.add(loci + k, 1);
+	return map_sets(st, mi, opt, seqs, lens, names, ls, 0, n_loci, n_reg_out, reg_out);
 }
 
 // ---------------------------------------------------------------- locus mode: the file driver
@@ -596,7 +674,7 @@ void LociFile::add_protein(const std::string &name, const std::string &seq)
 	names.push_back(name), seqs.push_back(seq);
 }
 
-int loci_file_read(const mp_idx_t *mi, const char *prot_fn, const char *loci_fn, LociFile &in)
+int loci_file_read(const mp_idx_t *mi, const char *prot_fn, const char *loci_fn, LociFile &in, bool by_set)
 {
 	if (!mi || !mi->nt || !prot_fn || !loci_fn) return -1;
 	{
@@ -620,6 +698,8 @@ int loci_file_read(const mp_idx_t *mi, const char *prot_fn, const char *loci_fn,
 	char *line = 0;
 	size_t cap = 0;
 	int rc = 0;
+	std::map<std::pair<int32_t, std::string>, int32_t> set_of; // by_set: (protein, label or "") -> set number, in order of first line
+	std::vector<int32_t> line_set;
 	for (long ln = 1; getline(&line, &cap, fp) >= 0; ++ln) {
 		std::vector<char*> t; // whitespace-separated fields
 		for (char *q = line; *q;) {
@@ -651,43 +731,57 @@ int loci_file_read(const mp_idx_t *mi, const char *prot_fn, const char *loci_fn,
 		mpb_locus_t l;
 		l.qid = in.qid[t[0]], l.cid = cid[t[1]], l.st = v[0], l.en = v[1];
 		in.loci.push_back(l);
+		if (by_set) line_set.push_back(set_of.emplace(std::make_pair(l.qid, std::string(t.size() >= 5 ? t[4] : "")), (int32_t)set_of.size()).first->second);
 	}
 	free(line);
 	fclose(fp);
 	if (rc != 0) return rc;
-	return check_loci(mi, (int32_t)in.seqs.size(), (int32_t)in.loci.size(), in.loci.data());
+	rc = check_loci(mi, (int32_t)in.seqs.size(), (int32_t)in.loci.size(), in.loci.data());
+	if (rc != 0) return rc;
+	in.by_set = by_set, in.sets = LocusSets();
+	if (!by_set) {
+		for (const mpb_locus_t &l : in.loci) in.sets.add(&l, 1);
+		return 0;
+	}
+	std::vector<std::vector<mpb_locus_t>> lines(set_of.size()); // the loci of each set, in file order
+	for (size_t k = 0; k < in.loci.size(); ++k) lines[(size_t)line_set[k]].push_back(in.loci[k]);
+	for (const std::vector<mpb_locus_t> &x : lines) in.sets.add(x.data(), (int64_t)x.size());
+	return 0;
 }
 
-// run_units over the pairs of a loci file, which are in memory already: units of at most mini_batch_size / n residues (at least one
-// pair), each aligned with map_loci.  Hits do not depend on unit boundaries (map_loci), so neither does the output.
+// run_units over the sets of a loci file, which are in memory already: units of whole sets, at most mini_batch_size / n residues (at
+// least one set), each aligned with map_sets.  Hits do not depend on unit boundaries (map_sets), so neither does the output.
 int32_t map_loci_file(Stages *const *st, int n, const mp_idx_t *mi, const LociFile &in, const mp_mapopt_t *opt, FILE *out)
 {
 	if (n < 1) return -1;
-	for (int k = 0; k < n; ++k)
+	const LocusSets &ls = in.sets;
+	const int32_t n_sets = ls.n();
+	for (int k = 0; k < n; ++k) {
 		if (!st[k]->loci_view(0, 0)) {
 			fprintf(stderr, "[miniprot_b200] this backend has no locus seeding stage\n");
 			return -3;
 		}
-	const int32_t n_loci = (int32_t)in.loci.size();
+		if (check_set_seeding(st[k], ls, 0, n_sets) != 0) return -3;
+	}
 	const int64_t unit_size = std::max<int64_t>(1, opt->mini_batch_size / n);
-	int32_t i0 = 0;
+	int32_t s = 0;
 	auto read = [&](bool &more) {
 		UnitPtr u;
-		if (i0 < n_loci) {
+		if (s < n_sets) {
 			u.reset(new Unit);
-			u->loci = in.loci.data() + i0;
-			for (int64_t residues = 0; i0 < n_loci && residues < unit_size; ++i0) {
-				const size_t q = (size_t)in.loci[(size_t)i0].qid;
+			u->sets = &ls, u->s0 = s;
+			for (int64_t residues = 0; s < n_sets && residues < unit_size; ++s) {
+				const size_t q = (size_t)ls.rng[(size_t)ls.off[(size_t)s]].qid;
 				residues += in.len[q];
 				u->sp.push_back(in.sp[q]), u->np.push_back(in.np[q]), u->len.push_back(in.len[q]);
 			}
 			u->n_reg.assign(u->len.size(), 0), u->reg.assign(u->len.size(), (mp_reg1_t*)0);
 		}
-		more = i0 < n_loci;
+		more = s < n_sets;
 		return u;
 	};
-	return run_units(st, n, mi, opt, out, "map_loci_file", "pairs", read, [&](Stages *s, int, Unit &u) {
-		u.rc = map_loci(s, mi, opt, (int32_t)in.seqs.size(), in.sp.data(), in.len.data(), in.np.data(), (int32_t)u.len.size(), u.loci, u.n_reg.data(), u.reg.data());
+	return run_units(st, n, mi, opt, out, in.by_set ? "map_locus_sets_file" : "map_loci_file", in.by_set ? "sets" : "pairs", read, [&](Stages *k, int, Unit &u) {
+		u.rc = map_sets(k, mi, opt, in.sp.data(), in.len.data(), in.np.data(), ls, u.s0, u.s0 + (int32_t)u.len.size(), u.n_reg.data(), u.reg.data());
 	});
 }
 

@@ -1,13 +1,15 @@
 """Throughput of locus mode (mpb_map_loci) on the C2 synthetic workload: each planted protein against its gene locus +- 10 kb.
 
-    python tools/loci_bench.py [--workload C2] [--flank 10000] [--repeats 3] [--ref-sample 20]
+    python tools/loci_bench.py [--workload C2] [--flank 10000] [--repeats 3] [--ref-sample 20] [--sets K]
 
 The loci come from a whole-genome mpb_map_batch of the same proteins (the primary hit of each protein, widened by the flank and
 clipped to its contig).  Reported, with the device name and power limit beside the numbers:
   * pairs/s of mpb_map_loci over all pairs in one call (the genome resident; best of the repeats);
   * proteins/s of the whole-genome mpb_map_batch of the same proteins (the k-mer index resident), for context;
   * loci/s of the reference CLI (oracle/_ref/miniprot, where it is built) run the way one maps a known locus without this library --
-    extract the locus to a FASTA, index it and map the protein, one run per locus -- on a sample of the loci, on the host.
+    extract the locus to a FASTA, index it and map the protein, one run per locus -- on a sample of the loci, on the host;
+  * with --sets K: each protein gets a locus set (mpb_map_locus_sets) of its gene locus plus the loci of the K - 1 proteins after it
+    as decoys; sets/s over all sets in one call, beside pairs/s of mpb_map_loci over the same (protein, locus) pairs.
 Inputs go to a temporary directory."""
 import argparse
 import json
@@ -51,6 +53,7 @@ def main():
     ap.add_argument("--flank", type=int, default=10_000)
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--ref-sample", type=int, default=20)
+    ap.add_argument("--sets", type=int, default=0, metavar="K", help="also time sets of each gene locus and K - 1 decoy loci")
     a = ap.parse_args()
     L = mp.lib()
     res = {"workload": a.workload, "flank": a.flank, **device_info()}
@@ -97,6 +100,24 @@ def main():
             mp.free_loci_regs(nr, rg)
         res["loci_pairs_per_s"] = round(len(loci) / min(times[1:]), 1)
         res["loci_bp_mean"] = round(sum(en - st for _, _, st, en in loci) / max(1, len(loci)))
+        if a.sets > 0:
+            sets = [[(q, c, st, en)] + [(q,) + loci[(i + j) % len(loci)][1:] for j in range(1, a.sets)] for i, (q, c, st, en) in enumerate(loci)]
+            pairs = [x for s in sets for x in s]
+            ts, tp = [], []
+            for _ in range(a.repeats + 1):
+                t0 = time.perf_counter()
+                rc, nr, rg = mp.map_locus_sets(ctx, mi, mo, seqs, names, sets)
+                ts.append(time.perf_counter() - t0)
+                assert rc == 0
+                mp.free_loci_regs(nr, rg)
+                t0 = time.perf_counter()
+                rc, nr, rg = mp.map_loci(ctx, mi, mo, seqs, names, pairs)
+                tp.append(time.perf_counter() - t0)
+                assert rc == 0
+                mp.free_loci_regs(nr, rg)
+            res["set_size"], res["sets"] = a.sets, len(sets)
+            res["locus_sets_per_s"] = round(len(sets) / min(ts[1:]), 1)
+            res["same_loci_pairs_per_s"] = round(len(pairs) / min(tp[1:]), 1)
         if os.path.exists(REF_BIN) and a.ref_sample > 0:
             genome = dict(read_fasta(g))
             ctg_names = [nt.ctg[i].name for i in range(nt.n_ctg)]

@@ -9,7 +9,12 @@ table, and the index options -k -M -L -b -T apply to a FASTA only (a .mpi file c
 TSV of `protein contig start end` (0-based, end exclusive, forward strand; both strands are searched).  Output comes in the order
 of the loci: PAF (columns 6-9 on the contig), or GFF3 / GTF (columns 1, 4 and 5 on the contig) with ids numbered over the whole
 file.  The options are the reference CLI's that mean something for one locus; -I (a max intron per locus) and --spsc are refused.
---devices 0,1 aligns on one GPU context per entry (repeats allowed); the output is the same."""
+--devices 0,1 aligns on one GPU context per entry (repeats allowed); the output is the same.
+
+--sets aligns each protein against all of its loci at once, as the reference aligns it against a genome made of those loci alone:
+hits across the loci are ranked together (one primary, the rest secondary; -N, -p, --outn, --outs and -u per set), and overlapping
+or abutting loci of one contig are merged.  An optional 5th column of LOCI labels the line's set: the lines of one protein and one
+label form one set, and without a label all lines of a protein do.  Sets come out in the order of their first line."""
 import argparse
 import ctypes as C
 import os
@@ -123,6 +128,7 @@ def parser() -> argparse.ArgumentParser:
     ap.add_argument("-I", action=_Apply, nargs=0, help="refused: " + REFUSED["-I"])
     ap.add_argument("--spsc", action=_Apply, help="refused: " + REFUSED["--spsc"], metavar="FILE")
     ap.add_argument("--devices", default="0", help="GPU contexts to align on, one per entry (repeats allowed) [0]")
+    ap.add_argument("--sets", action="store_true", help="align each (protein, 5th-column label) set of loci together, ranked as one genome")
     return ap
 
 
@@ -153,7 +159,7 @@ def main(argv=None):
     mi = mp.idx_load_genome(a.genome, io)
     ctxs = [mp.Context(d) for d in devices]
     try:
-        mp.map_loci_file(ctxs, mi, a.proteins, a.loci, "-", mo)
+        mp.map_loci_file(ctxs, mi, a.proteins, a.loci, "-", mo, sets=a.sets)
     except RuntimeError as e:
         sys.exit(str(e))
     finally:
